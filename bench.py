@@ -13,7 +13,8 @@ Default arm (this repo): 4096 tables per GPU (BASELINE configs[1]), random-init 
   e2e           libriichi.arena.OneVsThree.py_vs_py with a react_batch engine over lists of HOST numpy arrays (the plugin call)
   e2e_with_net  the same through DeviceEngine.react_batch (np.stack -> H2D -> 192x40 net -> lists), i.e. the `value` workload
   shanten_1m / agari_1m / encode_65536   BASELINE configs[2] and [3]
-  cpu_baseline  the CPU oracle on this box's host cores, bounded sample (rank 0, N=1 only)
+  cpu_baseline  the CPU oracle on this machine's host cores, bounded sample (rank 0, N=1 only)
+`--dump-outputs DIR` writes what the `value` path computed in its last timed step (see LastDecisionRecorder).
 `--impl reference` times libriichi's own CPU path restated by the oracle (oracle/, all host threads): the same 4096 tables, the
 same policy (kind 2) and therefore the same games as `env_only` and `e2e`.
 """
@@ -35,6 +36,7 @@ SEED_START = (10000, 0x2000)  # mortal/player.py:67
 OBS_BYTES = 1012 * 34 * 4
 MASK_BYTES = 46
 STATE_BYTES = 1952  # sizeof(TableState) read per encoded row
+H100_HBM_GBS = 3350.0  # H100 SXM data sheet; MEASURED_PEAKS.json hbm_gbs replaces it when present
 
 
 def host_cores() -> int:
@@ -45,11 +47,12 @@ def host_cores() -> int:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons / power limit DURING the timed region (a number is only worth something with the
+    clock and power limit it was measured at)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-         "clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, gpu_index: int):
         self.gpu = gpu_index
@@ -73,22 +76,23 @@ class ClockSampler:
 
     def stop(self):
         if self.proc is None:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return {"sm_mhz": None, "sm_max_mhz": None, "power_limit_w": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.25)
         self.proc.terminate()
         try:
             self.proc.wait(timeout=2)
         except Exception:
             self.proc.kill()
-        sm, mx, reasons = [], [], set()
+        sm, mx, plim, reasons = [], [], [], set()
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for s in self.samples:
             f = [x.strip() for x in s.split(",")]
-            if len(f) < 8:
+            if len(f) < 9:
                 continue
             try:
                 sm.append(float(f[1]))
                 mx.append(float(f[2]))
+                plim.append(float(f[8]))
             except ValueError:
                 continue
             for name, v in zip(names, f[4:8]):
@@ -96,7 +100,7 @@ class ClockSampler:
                     reasons.add(name)
         sm.sort()
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "reasons": sorted(reasons), "samples": len(sm)}
+                "power_limit_w": min(plim) if plim else None, "reasons": sorted(reasons), "samples": len(sm)}
 
 
 def seeds_for_rank(rank: int, n_tables: int):
@@ -164,7 +168,7 @@ def workload_config(world, args):
     return {"workload": "BatchGame 4096 tables/GPU, random-init Mortal brain (192ch x 40 blocks, v4 obs), self-play step loop (BASELINE configs[1])",
             "tables_per_gpu": N_TABLES, "global_tables": N_TABLES * world, "obs_version": 4,
             "seed_start": list(SEED_START), "fast_forward_steps": args.skip, "parallelism": f"tables sharded dp{world}, no data-path collective",
-            "l2": "per-step obs output (~0.56 GB) exceeds the 126 MB L2, no explicit flush",
+            "l2": "per-step obs output (~0.56 GB) exceeds the 50 MB L2, no explicit flush",
             "sp_block": "rows 889-1011 (single-player tables) computed on device by the k_sp_* kernels"}
 
 
@@ -301,6 +305,54 @@ class HostNetEngine:
         return self.e.react_batch(obs, masks, invisible_obs)
 
 
+class LastDecisionRecorder:
+    """--dump-outputs: stands in for the DeviceEngine inside the arena of the `value` path and keeps device copies of what the
+    last timed cycle's react_static call received (the legal masks, an evenly spaced fixed sample of the observation rows) and
+    returned to the arena (actions, Q-values). Copies are device-side and asynchronous; nothing reaches the host before the
+    timed window has closed. The Q-values of illegal actions are -inf by construction (DQN), so only the legal ones are written:
+    q_values_legal = q[masks], row-major, which masks.npy locates.
+    k_step hands out decision rows with an atomic counter, so the position of a row in the batch changes from run to run while
+    its content does not: every array is written in the order of the row's (table, seat, kan-select) key, stored beside it."""
+
+    OBS_SAMPLE_ROWS = 64  # 64 x 1012 x 34 f32 = 8.8 MB
+
+    def __init__(self, engine):
+        self.engine = engine
+        self.armed = False
+        self.env = None  # the arena's BatchEnv: row_table / row_seat of the rows react_static is handed
+        self.out = None
+
+    def __getattr__(self, name):
+        return getattr(self.engine, name)
+
+    def react_static(self, obs_buf, masks_buf, nr):
+        import torch
+
+        a, q = self.engine.react_static(obs_buf, masks_buf, nr)
+        if self.armed:
+            table, rs = self.env.row_table[:nr].long(), self.env.row_seat[:nr].long()
+            order = torch.argsort(table * 8 + rs)  # unique per row: table, seat (bits 0-1), kan-select (bit 2)
+            k = min(nr, self.OBS_SAMPLE_ROWS)
+            pos = torch.arange(k, device=obs_buf.device) * nr // k  # evenly spaced positions in that order
+            self.out = {"table": table[order], "seat": rs[order] & 3, "kan_select": (rs[order] >> 2) & 1, "actions": a[order],
+                        "q_values": q[order], "masks": masks_buf[:nr][order], "obs_sample": obs_buf.index_select(0, order[pos]),
+                        "obs_sample_rows": pos}
+        return a, q
+
+    def dump(self, out_dir):
+        """DIR/<name>.npy, float32 (float64 for the integer arrays: exact)"""
+        import numpy as np
+
+        out = {name: t.cpu().numpy() for name, t in self.out.items()}
+        out["q_values_legal"] = out.pop("q_values")[out["masks"]]
+        os.makedirs(out_dir, exist_ok=True)
+        for name, arr in out.items():
+            arr = arr.astype(np.float64 if name in ("table", "seat", "kan_select", "actions", "obs_sample_rows") else np.float32)
+            if not np.isfinite(arr).all():
+                raise RuntimeError(f"--dump-outputs: {name} has non-finite entries")
+            np.save(os.path.join(out_dir, f"{name}.npy"), arr)
+
+
 def run_ours(args):
     import numpy as np
     import torch
@@ -401,7 +453,7 @@ def run_ours(args):
 
     # -------- the product path: libriichi.arena.OneVsThree.py_vs_py (for host-protocol engines two half-batches stepped alternately:
     # kernels + D2H of one half overlap the engine's host work on the other), timed between two cycle hooks
-    def run_arena(agent, n_warm, n_timed, pipeline=True):
+    def run_arena(agent, n_warm, n_timed, pipeline=True, recorder=None):
         arena = OneVsThree(disable_progress_bar=True, device=local_rank)
         arena.pipeline = pipeline
         arena.fast_forward_steps = args.skip
@@ -413,10 +465,14 @@ def run_ours(args):
             if c in (n_warm, n_warm + n_timed):
                 torch.cuda.synchronize()
                 marks[c] = (time.perf_counter(), state.total_steps(), rows())
+            if recorder is not None:
+                recorder.armed = c == n_warm + n_timed - 1  # the last timed cycle
+                recorder.env = state.parts[0].env
 
         arena.cycle_hook = hook
         # same tables as the other loops: rank r starts at seed_start + 1024 r
-        arena.py_vs_py(agent, agent, (int(nonces[0]), int(keys[0])), N_TABLES // 4)
+        player = agent if recorder is None else recorder
+        arena.py_vs_py(player, player, (int(nonces[0]), int(keys[0])), N_TABLES // 4)
         (t0, s0, r0), (t1, s1, r1) = marks[n_warm], marks[n_warm + n_timed]
         return dict(ms=(t1 - t0) * 1000.0, table_steps=s1 - s0, rows=r1 - r0, n=n_timed, launches=arena.last_stats["launches"],
                     cycles=arena.last_stats["cycles"])
@@ -433,8 +489,11 @@ def run_ours(args):
     a_nn_ms = sum(e[1].elapsed_time(e[2]) for e in a_split) / K
     ea[0].close()
     barrier()
-    av = run_arena(engine, W, K)  # the headline `value`: the same workload through the arena (pipelined half-batches)
+    recorder = LastDecisionRecorder(engine) if args.dump_outputs else None
+    av = run_arena(engine, W, K, recorder=recorder)  # the headline `value`: the same workload through the arena
     barrier()
+    if recorder is not None and rank == 0:
+        recorder.dump(args.dump_outputs)
     clocks = sampler.stop()
 
     # -------- loop B: env only (test policy on device, no host sync); B2 = the same with the single-player block off
@@ -482,8 +541,7 @@ def run_ours(args):
     barrier()
     cn = None
     if not args.no_e2e_net:
-        kn = max(3, min(K, args.e2e_net_steps))
-        cn = run_e2e(HostNetEngine(engine), max(W, 4), kn)
+        cn = run_e2e(HostNetEngine(engine), max(W, 4), K if args.e2e_net_steps is None else args.e2e_net_steps)
         barrier()
     # what the link gives for the same bytes: one plain pinned D2H copy (context for e2e, not a claim)
     nprobe = max(1, c["rows"] // K)
@@ -549,14 +607,8 @@ def run_ours(args):
                 peaks = json.load(f)
         except Exception:
             pass
-        peak_gbs = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6.65 TB/s"
-        traffic = {}
-        try:  # dram__bytes_read + dram__bytes_write per launch, from the committed ncu --set full summaries
-            with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-                traffic = json.load(f)
-        except Exception:
-            pass
+        peak_gbs = float(peaks.get("hbm_gbs", H100_HBM_GBS))
+        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3.35 TB/s"
         rows_per_launch = b_rows / K
         bytes_per_launch = rows_per_launch * (OBS_BYTES + MASK_BYTES + STATE_BYTES)
         gbs = lambda ms: bytes_per_launch / (ms / K * 1e-3) / 1e9 if ms > 0 else 0.0
@@ -570,8 +622,8 @@ def run_ours(args):
             "step_breakdown_ms": {"env": a_env_ms, "policy_net": a_nn_ms, "sequential_total": a_ms / K, "pipelined_total": av_ms / K,
                                   "note": "`value` runs OneVsThree.py_vs_py with the DeviceEngine for all seats (one batch, one stream, CUDA-graph "
                                           "forward); env / policy_net split the same workload driven by bench.py's own loop (CUDA events), whose "
-                                          "throughput is value_sequential. Two half-batches on two streams were measured SLOWER for device engines "
-                                          "(208 K vs 252 K table-steps/s): the arena pipelines half-batches for host-protocol engines only (e2e)"},
+                                          "throughput is value_sequential. The arena pipelines two half-batches on two streams for "
+                                          "host-protocol engines only (e2e)"},
             "value_sequential": a_units / (a_ms * 1e-3),
             "env_only": {"value": b_units / (b_ms * 1e-3), "unit": "table-steps/s", "ms_per_step": b_ms / K,
                          "policy": "device test policy kind 2 (mask-hash; the CPU arm's and the e2e engine's policy), no host sync",
@@ -583,11 +635,10 @@ def run_ours(args):
             # alone and the encoder pair without the single-player DP.
             "roofline": {"kernel": "v4 encode_obs: k_encode_features + k_encode_store + k_sp_* (single-player tables)", "bound": "hbm",
                          "achieved": gbs(full_ms), "peak": peak_gbs, "unit": "GB/s", "frac": gbs(full_ms) / peak_gbs,
-                         "traffic": traffic.get("encode_full"), "peak_source": peak_src, "bytes_per_launch": bytes_per_launch,
+                         "peak_source": peak_src, "bytes_per_launch": bytes_per_launch,
                          "ms_per_launch": full_ms / K, "rows_per_launch": rows_per_launch,
                          "kernels": {
-                             "k_encode_store": {"ms_per_launch": store_ms / K, "achieved": gbs(store_ms), "frac": gbs(store_ms) / peak_gbs,
-                                                "traffic": traffic.get("k_encode_store")},
+                             "k_encode_store": {"ms_per_launch": store_ms / K, "achieved": gbs(store_ms), "frac": gbs(store_ms) / peak_gbs},
                              "k_encode_features": {"ms_per_launch": feat_ms / K},
                              "encoder_pair": {"ms_per_launch": (feat_ms + store_ms) / K, "achieved": gbs(feat_ms + store_ms),
                                               "frac": gbs(feat_ms + store_ms) / peak_gbs},
@@ -612,7 +663,7 @@ def run_ours(args):
             # this library's kernels in the timed region: env kernels counted by libmjx, plus the fused policy-net kernels
             # (4 per residual block + 1, csrc/mjx_nn.cuh) that each CUDA-graph replay of the forward contains
             "gpu_launches": int(av["launches"] * K / max(av["cycles"], 1)) + 2 * K * (4 * 40 + 1), "gpu_launches_env": a["launches"], "clocks": clocks,
-            "collective": collective,
+            "collective": collective, "gpu": torch.cuda.get_device_name(dev),
         }
         line.update(extras)
         if world == 1 and not args.no_cpu_baseline:
@@ -659,7 +710,7 @@ def bench_encode_64k(mortal_b200, torch, np, dev, local_rank):
     env.close()
     del obs64
     torch.cuda.empty_cache()
-    peak = 6650.0
+    peak = H100_HBM_GBS
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             peak = float(json.load(f).get("hbm_gbs", peak))
@@ -685,7 +736,7 @@ def bench_algo_1m(torch, np, dev, args):
     d_t, d_l = torch.from_numpy(tiles).to(dev), torch.from_numpy(lens).to(dev)
     d_o = torch.empty(n, dtype=torch.int8, device=dev)
     st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-    # the 34 MB of hands would stay in the 126 MB L2 between repetitions: rotate through 8 copies (272 MB) so every launch reads HBM
+    # the 34 MB of hands would stay in the 50 MB L2 between repetitions: rotate through 8 copies (272 MB) so every launch reads HBM
     d_ts = [d_t] + [d_t.clone() for _ in range(7)]
     rot = [0]
 
@@ -753,11 +804,13 @@ def main():
     ap.add_argument("--skip", type=int, default=300, help="untimed fast-forward batch steps before warm-up (both arms)")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--cpu-baseline-steps", type=int, default=12, help="timed batch steps of the cpu_baseline leg of the default arm")
-    ap.add_argument("--e2e-net-steps", type=int, default=12)
+    ap.add_argument("--e2e-net-steps", type=int, default=None, help="timed steps of the e2e_with_net leg (default: --steps)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e-net", action="store_true")
     ap.add_argument("--no-algo-1m", action="store_true", help="skip BASELINE configs[2] (shanten / agari at 1M hands)")
     ap.add_argument("--no-encode-64k", action="store_true", help="skip the BASELINE configs[3] encode measurement (27 GB obs buffer)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the actions, legal Q-values, legal masks and a fixed sample of the observations of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3

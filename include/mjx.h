@@ -1,8 +1,8 @@
-/* mjx — C ABI of the B200-native batched riichi self-play environment (libmjx.so).
+/* mjx — C ABI of the H100-native batched riichi self-play environment (libmjx.so).
  *
  * This is the drop-in boundary for libriichi's self-play hot path. libriichi has no C ABI of its
  * own (it is Rust re-exported through PyO3); each entry point below names the reference interface
- * it stands in for (paths relative to /root/reference/libriichi/src). Plain pointers and sizes only;
+ * it stands in for (paths relative to Mortal's libriichi/src). Plain pointers and sizes only;
  * "dev" pointers are CUDA device pointers (e.g. torch.Tensor.data_ptr()), "host" pointers are
  * ordinary host memory; `stream` is a cudaStream_t passed as void* (NULL = legacy default stream).
  * Every function returns 0 on success or a negative mjx_status; mjx_last_error() gives the text.

@@ -106,7 +106,7 @@ def load():
     path = lib_path()
     if not os.path.exists(path):
         raise MjxError(f"{path} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                       "(nvcc, sm_100a). mortal_b200 has no CPU fallback.")
+                       "(nvcc, sm_90a). mortal_b200 has no CPU fallback.")
     L = C.CDLL(path)
     for name, (res, args) in SYMBOLS.items():
         fn = getattr(L, name)  # AttributeError if the library does not export a declared symbol

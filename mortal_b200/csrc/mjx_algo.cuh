@@ -1,4 +1,4 @@
-// mortal_b200 — device-side shanten / agari / point (sm_100a).
+// mortal_b200 — device-side shanten / agari / point (sm_90a).
 // Behavioural contract: libriichi algo/shanten.rs:88-150, algo/agari.rs:203-285 & 287-761 & 767-912,
 // algo/point.rs:13-112. Implementation is this repo's own: packed 40-bit table rows gathered from
 // L2, a fully unrolled min-plus merge in registers, incremental chiitoi/kokushi signatures so that a

@@ -1,4 +1,4 @@
-// mortal_b200 — CUDA kernels (sm_100a) and the C ABI of include/mjx.h.
+// mortal_b200 — CUDA kernels (sm_90a) and the C ABI of include/mjx.h.
 #include <cstdio>
 #include <cstring>
 #include <mutex>
@@ -539,7 +539,7 @@ thread_local std::string g_err;
 std::mutex g_mu;
 bool g_ready = false;
 int g_device = -1;
-int g_sm_count = 148;
+int g_sm_count = 0;  // mjx_init reads it from the device
 Tables g_T;
 const float* g_sp_p_tab = nullptr;  // csrc/mjx_sp.cuh draw-probability table (device)
 

@@ -1,5 +1,5 @@
 // mortal_b200 — fused elementwise kernels for the policy-net inference path (mortal/model.py ResBlock / ChannelAttention,
-// restated in mortal_b200/model.py). The convolutions stay with cuDNN (tcgen05 implicit-GEMM kernels); what PyTorch runs
+// restated in mortal_b200/model.py). The convolutions stay with cuDNN (implicit-GEMM kernels); what PyTorch runs
 // between them as 5-6 separate bandwidth-bound passes per block (BatchNorm affine, Mish, two pooling reductions, gate
 // multiply, residual add) is done here in three: one 16-byte vector of 8 bf16 channels per thread, NHWC
 // (channels-last) activations [B, L, C], fp32 math, one rounding to bf16 at the end.

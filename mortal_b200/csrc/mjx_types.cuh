@@ -1,4 +1,4 @@
-// mortal_b200 — B200-native batched riichi environment (sm_100a).
+// mortal_b200 — H100-native batched riichi environment (sm_90a).
 // Table record layout in HBM and small tile helpers.
 //
 // One table = one 16-byte-aligned record. A warp owns a table: it loads the record into shared

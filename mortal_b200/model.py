@@ -4,7 +4,7 @@ Architecture restated from mortal/model.py:10-231 (version 4): Conv1d stem -> `n
 residual blocks (BN -> Mish -> Conv1d k3, twice) each gated by a squeeze/excite style channel attention
 -> BN -> Mish -> Conv1d(C, 32, k3) -> Mish -> Linear(32*34, 1024) -> Mish ; dueling head Linear(1024, 1+46)
 with the advantage mean taken over legal actions only and illegal actions at -inf. Real Mortal checkpoints
-load into mortal/model.py unchanged; this module exists so bench.py does not depend on /root/reference.
+load into mortal/model.py unchanged; this module exists so bench.py does not depend on the reference checkout.
 """
 from __future__ import annotations
 

@@ -4,7 +4,7 @@
 // __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs do.
 //
 // Every function cites the reference file:line (relative to
-// /root/reference/libriichi/src) whose behaviour it restates.
+// Mortal's libriichi/src) whose behaviour it restates.
 #pragma once
 #include <cstdint>
 #include <cstring>

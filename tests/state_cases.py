@@ -1,4 +1,4 @@
-"""The assertions of the reference's state tests (/root/reference/libriichi/src/state/test.rs, line refs inline), written
+"""The assertions of the reference's state tests (Mortal's libriichi/src/state/test.rs, line refs inline), written
 against the libriichi.state.PlayerState surface so that the same bodies run on the oracle (tests/test_oracle_state.py keeps its
 own copy), on the host-emulated product (tests/test_emul_state.py) and on the CUDA path (tests/test_gpu_state.py).
 Inline mjai logs: tests/golden/state_test_logs.json (tools/extract_ref_fixtures.py)."""

@@ -354,49 +354,51 @@ def test_arena_host_protocol_loop_on_emulated_env_fail_fast():
     assert (ref["scores"] == arena.last_results["scores"]).all() and (ref["ranks"] == arena.last_results["ranks"]).all()
 
 
-def test_reference_mortal_engine_and_model_drop_in_unchanged():
-    """north_star: "mortal/train.py and mortal/engine.py drop in unchanged". The reference's OWN, unmodified mortal/engine.py
-    (MortalEngine) and mortal/model.py (Brain, DQN) are imported from /root/reference against the `libriichi` module this repo
-    installs, and drive libriichi.arena.OneVsThree.py_vs_py exactly like mortal/player.py:60-69 does (host-emulated environment:
-    this container has no GPU). The recorded decisions replay in the oracle to the same scores / rankings. Skipped where the
-    reference tree is absent (the GPU box)."""
-    import importlib
-    import sys
+def test_reference_engine_game_replays_through_the_arena():
+    """north_star: "mortal/train.py and mortal/engine.py drop in unchanged". tests/golden/reference_engine_game.json.gz records the
+    reference's own, unmodified mortal/engine.py (MortalEngine) and mortal/model.py (Brain, DQN) driving
+    libriichi.arena.OneVsThree.py_vs_py of this repository like mortal/player.py:60-69 does (host-emulated environment; made by
+    tools/extract_ref_fixtures.py): a digest of the observations and masks of every engine call and the actions returned. Two
+    reference-protocol engines replay those answers here: every call must hand them the same rows, the games must end with the
+    recorded results, and the recorded decisions must replay in the oracle to the same scores / rankings."""
+    import gzip
+    import json
 
-    import pytest
+    sys.path.insert(0, os.path.join(ROOT, "tools"))
+    from extract_ref_fixtures import rows_digest
 
-    ref_dir = "/root/reference/mortal"
-    if not os.path.isdir(ref_dir):
-        pytest.skip("reference tree not present")
-    import torch
+    from mortal_b200.libriichi.arena import OneVsThree
 
-    import mortal_b200.libriichi as lr
+    with gzip.open(os.path.join(ROOT, "tests", "golden", "reference_engine_game.json.gz"), "rt") as f:
+        gold = json.load(f)
 
-    lr.install()
-    sys.path.insert(0, ref_dir)
-    try:
-        for name in ("model", "engine"):
-            sys.modules.pop(name, None)
-        ref_model = importlib.import_module("model")
-        ref_engine = importlib.import_module("engine")
-    finally:
-        sys.path.remove(ref_dir)
-    assert ref_model.__file__.startswith(ref_dir) and ref_engine.__file__.startswith(ref_dir)
-    from libriichi.arena import OneVsThree
+    class Replay:
+        engine_type = "mortal"; version = 4; is_oracle = False; enable_quick_eval = True; enable_rule_based_agari_guard = False
 
-    torch.manual_seed(0)
-    mk = lambda name: ref_engine.MortalEngine(ref_model.Brain(version=4, conv_channels=16, num_blocks=1).eval(),
-                                              ref_model.DQN(version=4).eval(), is_oracle=False, version=4,
-                                              device=torch.device("cpu"), enable_amp=False, enable_quick_eval=True,
-                                              enable_rule_based_agari_guard=False, name=name)
+        def __init__(self, name):
+            self.name, self.calls, self.n = name, gold["calls"][name], 0
+
+        def react_batch(self, obs, masks, invisible_obs):
+            call = self.calls[self.n]
+            self.n += 1
+            assert rows_digest(obs, masks) == call["rows_sha256"], f"{self.name} call {self.n - 1}: other rows than the reference engine saw"
+            assert len(call["actions"]) == len(obs)
+            return call["actions"], [[0.0] * 46 for _ in obs], [list(m) for m in masks], [True] * len(obs)
+
+    challenger, champion = Replay("challenger"), Replay("champion")
     arena = _emul_arena(OneVsThree)
     arena.record_decisions = True
-    rankings = arena.py_vs_py(challenger=mk("challenger"), champion=mk("champion"), seed_start=(10000, 0x2000), seed_count=1)
-    assert sum(rankings) == 4
+    rankings = arena.py_vs_py(challenger=challenger, champion=champion, seed_start=tuple(gold["seed_start"]), seed_count=gold["seed_count"])
+    assert challenger.n == len(challenger.calls) and champion.n == len(champion.calls)
+    assert rankings == gold["rankings"] and sum(rankings) == 4
+    got = arena.last_results
+    for k in ("scores", "ranks", "steps"):
+        assert (got[k] == np.array(gold[k])).all(), k
+    assert (arena.last_decisions == np.array(gold["decisions"])).all()
+    assert (arena.last_decision_masks == np.array(gold["decision_masks"])).all()
     nonces = np.repeat(np.arange(10000, 10001, dtype=np.uint64), 4)
     keys = np.full(4, 0x2000, dtype=np.uint64)
     ref = O.run_replay(nonces, keys, arena.last_decisions, quick_eval=True, mask_bits=arena.last_decision_masks)
-    got = arena.last_results
     assert (ref["scores"] == got["scores"]).all() and (ref["ranks"] == got["ranks"]).all() and (ref["steps"] == got["steps"]).all()
     hist = [0, 0, 0, 0]
     for i in range(4):

@@ -1,6 +1,6 @@
 """Pins the oracle's algo layer to the reference's own known-answer tests.
 
-Transcribed from /root/reference/libriichi/src: algo/shanten.rs:157-202, algo/agari.rs:919-1380,
+Transcribed from Mortal's libriichi/src: algo/shanten.rs:157-202, algo/agari.rs:919-1380,
 algo/point.rs:120-154, rankings.rs:29-66.
 """
 import numpy as np

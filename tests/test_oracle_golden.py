@@ -1,7 +1,7 @@
 """Replays the reference's only seeded full-game log through the oracle, end to end.
 
 Fixture: tests/golden/golden_game.jsonl, extracted by tools/extract_ref_fixtures.py from
-/root/reference/log-viewer/index.example.html:10-264 (seed [10637, 12210010324280706444]).
+Mortal's log-viewer/index.example.html:10-264 (seed [10637, 12210010324280706444]).
 Pins: SHA3/ChaCha12/rand-0.8 shuffle + wall slicing (every haipai, tsumo, dora, ura marker),
 PlayerState legal-action masks (`meta.mask_bits` of every logged decision), riichi sticks,
 honba/kyotaku payout, hora deltas, scores at each start_kyoku and the tobi ending.

@@ -1,6 +1,6 @@
 """Pins the oracle's PlayerState to the reference's state tests.
 
-Assert logic re-stated from /root/reference/libriichi/src/state/test.rs (line refs inline); the inline
+Assert logic re-stated from Mortal's libriichi/src/state/test.rs (line refs inline); the inline
 mjai logs come from tests/golden/state_test_logs.json (tools/extract_ref_fixtures.py).
 Every update is followed by the reference's own invariant checker (test.rs:49-67).
 """

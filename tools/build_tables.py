@@ -1,14 +1,14 @@
 #!/usr/bin/env python
-"""Build the lookup tables used by both the oracle and the CUDA library into mortal_b200/data/ (git-ignored, travels
-to the GPU box like a built .so).
+"""Build the lookup tables used by both the oracle and the CUDA library into mortal_b200/data/ (git-ignored build
+products, like the built .so).
 
 * shanten_suhai.bin / shanten_jihai.bin are GENERATED from first principles by tools/gen_shanten_tables.cc (a DP over
   the rank counts; no input files) and truncated to the row counts of libriichi's tables (1,940,777 / 78,032 rows:
   indices past the end read as an all-zero row in the reference, algo/shanten.rs:52, and that quirk is part of the
-  contract). When the reference tree is present the result is checked byte for byte against its data files.
+  contract). The result is checked byte for byte against libriichi's data files (tests/golden/tables/).
 * agari.bin (9,362 keys) is GENERATED from first principles by tools/gen_agari_table.py (enumeration of all hand shapes
-  that split into melds + pair or seven pairs; no input files). Records are written in ascending key order; when the
-  reference tree is present the result is checked against libriichi's data file as key -> ordered div list (the
+  that split into melds + pair or seven pairs; no input files). Records are written in ascending key order; the result
+  is checked against libriichi's data file (tests/golden/tables/) as key -> ordered div list (the
   reference loads its file into a hash map, agari.rs:22-51, so the order of records is not content).
 Nothing is copied from the reference any more. Formats: SURVEY.md Appendix A.
 """
@@ -18,8 +18,9 @@ import subprocess
 import sys
 import tempfile
 
-REF = os.environ.get("MORTAL_REF_DATA", "/root/reference/libriichi/src/algo/data")
-OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "mortal_b200", "data")
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+REF = os.path.join(ROOT, "tests", "golden", "tables")  # libriichi's data files, for the check
+OUT = os.path.join(ROOT, "mortal_b200", "data")
 FILES = {
     "shanten_suhai.bin": ("shanten_suhai.bin.gz", 9_703_885),
     "shanten_jihai.bin": ("shanten_jihai.bin.gz", 390_160),

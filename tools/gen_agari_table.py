@@ -24,7 +24,7 @@ table's content is part of the contract (the oracle and the CUDA library must se
 * a seven-pairs shape that also splits into melds (two double runs) carries no seven-pairs flag.
 
 File order: ascending key (the reference loads its file into a hash map, so the order of its records is not content).
-`tests/test_tables.py` compares key -> ordered div list with libriichi's data file whenever the reference tree is present.
+`tests/test_tables.py` compares key -> ordered div list with libriichi's data file (tests/golden/tables/agari.bin.gz).
 """
 import itertools
 import struct

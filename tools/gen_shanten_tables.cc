@@ -6,8 +6,8 @@
 // of a tile. These are the "distance" tables of the table-based shanten algorithm libriichi uses (algo/shanten.rs:27-84,
 // 88-100: the per-suit rows are combined by a min-plus merge and 1 is subtracted at the end).
 // Output format = the reference's unpacked table: 5 bytes per row, low nibble first (shanten.rs:27-44).
-// tools/build_tables.py runs this and cross-checks the result byte for byte against the reference's own data files
-// whenever /root/reference is present (tests/test_tables.py).
+// tools/build_tables.py runs this and cross-checks the result byte for byte against the reference's own data files,
+// stored in tests/golden/tables/ (tests/test_tables.py).
 #include <algorithm>
 #include <cstdint>
 #include <cstdio>
