@@ -144,6 +144,49 @@ int mjx_env_replay_trust_seeds(mjx_env* env, const uint64_t* nonces_host, const 
 int64_t* mjx_env_row_label(mjx_env* env); /* int64 [row_cap] device */
 uint8_t* mjx_env_row_meta(mjx_env* env);  /* uint8 [row_cap, 4] device: at_kyoku, at_turn, shanten (int8), apply_gamma */
 
+/* ---- log validation: bin/validate_logs.rs:62-242 process_path ---------------------------------------------------------
+ * Replays every log through the four seats (state/update.rs update_with_keep_cans(ev, true)) and reports the first event a rule
+ * forbids. Inputs are host arrays in the mjx_env_create_replay layout (`hdr`, `ev_off`, `ev_cnt`, `kyoku`, `ky_off`; one entry per
+ * log) plus the hora side array: MJX_HORA_WORDS words per hora event, log i's first entry at hora_off[i]:
+ *   word 0 = (uint32) deltas[actor] | has_deltas << 32 | has_ura << 33 | n_ura << 36,  word 1 = ura tiles, one byte each.
+ * out_verdicts: host mjx_verdict [n_logs]. One launch (one warp per log); blocking. */
+#define MJX_HORA_WORDS 2
+enum mjx_verdict_status { MJX_V_OK = 0, MJX_V_CHECK = 1, MJX_V_UPDATE = 2, MJX_V_PARSE = 3, MJX_V_UNSUPPORTED = 4 };
+/* The reasons a verdict can carry: X(enum suffix, name). The CHECK reasons are the 19 checks of process_path in order; UPDATE
+ * the errors of PlayerState::update_with_keep_cans (plus a caught panic); PARSE the host-side rejections; UNSUPPORTED an event
+ * this implementation's table record cannot hold. This list is the single definition (mortal_b200/validate_logs.py reads it). */
+#define MJX_VALIDATE_REASONS(X)                                                                                              \
+    X(NONE, "none")                                                                                                          \
+    X(CAN_DISCARD, "can_discard") X(DISCARD_CANDIDATES, "discard_candidates") X(CHI_NON_KAMICHA, "chi from non-kamicha")     \
+    X(CAN_CHI_LOW, "can_chi_low") X(CAN_CHI_MID, "can_chi_mid") X(CAN_CHI_HIGH, "can_chi_high") X(CAN_PON, "can_pon")        \
+    X(CAN_DAIMINKAN, "can_daiminkan") X(CAN_ANKAN, "can_ankan") X(ANKAN_CANDIDATES, "ankan_candidates")                      \
+    X(CAN_KAKAN, "can_kakan") X(KAKAN_CANDIDATES, "kakan_candidates") X(CAN_RIICHI, "can_riichi")                            \
+    X(CAN_RON_AGARI, "can_ron_agari") X(CAN_TSUMO_AGARI, "can_tsumo_agari") X(MISSING_URA, "missing ura_markers")            \
+    X(MISSING_DELTAS, "missing deltas") X(AGARI_POINTS, "agari_points") X(DELTAS_BELOW_POINTS, "deltas below points")       \
+    X(EXHAUSTED_YAMA, "tsumo from exhausted yama") X(UNKNOWN_TILE, "witness unknown tile")                                   \
+    X(FIFTH_TILE, "witness fifth tile") X(DISCARD_FROM_VOID, "discard from void") X(CONSUME_FROM_VOID, "consume from void")  \
+    X(DORA_OVERFLOW, "dora indicator overflow") X(UPDATE_OTHER, "other")                                                     \
+    X(PARSE_JSON, "json") X(PARSE_TYPE, "unknown type") X(PARSE_TILE, "unknown tile") X(PARSE_ACTOR, "actor out of range")  \
+    X(PARSE_CONSUMED, "consumed length") X(PARSE_FIELD, "missing or invalid field")                                          \
+    X(CAPACITY, "capacity")
+#define MJX_REASON_ENUM_(id, name) MJX_R_##id,
+enum mjx_validate_reason { MJX_VALIDATE_REASONS(MJX_REASON_ENUM_) MJX_R_COUNT };
+#undef MJX_REASON_ENUM_
+typedef struct mjx_verdict {
+    int32_t status;  /* mjx_verdict_status */
+    int32_t reason;  /* mjx_validate_reason */
+    int32_t line;    /* 1-based event index of the failure (0 when OK) */
+    int32_t seat;    /* UPDATE: the lowest seat whose update fails; CHECK: the actor; else -1 */
+} mjx_verdict;
+int mjx_validate_logs(int n_logs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt, long long n_hdr,
+                      const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words, const uint64_t* hora_payload,
+                      const int32_t* hora_off, long long n_hora_words, mjx_verdict* out_verdicts, void* stream);
+/* The same over device arrays, enqueued on `stream` without a synchronise (out_verdicts: device mjx_verdict [n_logs]). A log whose
+ * event range lies outside the word array gets an UNSUPPORTED verdict instead of being read. */
+int mjx_validate_logs_dev(int n_logs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt, long long n_hdr,
+                          const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words, const uint64_t* hora_payload,
+                          const int32_t* hora_off, long long n_hora_words, mjx_verdict* out_verdicts, void* stream);
+
 /* ---- libriichi.state.PlayerState (state/player_state.rs:143-264, state/getter.rs:6-156, state/obs_repr.rs:776-791) ---------
  * A batch of n independent single-seat states: table records in single-seat mode (other seats' hidden tiles are `?` = 37), updated
  * by the same device event handlers self-play uses. `mjx_state_create` returns an mjx_env whose encoder entry points

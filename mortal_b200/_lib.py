@@ -95,6 +95,10 @@ SYMBOLS = {
     "mjx_shanten_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "mjx_agari_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "mjx_make_wall_host": (C.c_int, [C.c_uint64, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "mjx_validate_logs": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong,
+                                    C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p]),
+    "mjx_validate_logs_dev": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p,
+                                        C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p]),
 }
 
 

@@ -9,6 +9,7 @@
 #include "mjx_sp.cuh"
 #include "mjx_policy.cuh"
 #include "mjx_replay.cuh"
+#include "mjx_validate.cuh"
 #include "mjx_invisible.cuh"
 #include "mjx_state.cuh"
 #include "mjx_nn.cuh"
@@ -79,6 +80,32 @@ __global__ void __launch_bounds__(STEP_WARPS * 32) k_replay_step(EnvView V, Repl
     uint4* gdst = reinterpret_cast<uint4*>(g);
     for (int i = lane; i < NV; i += 32) gdst[i] = dst[i];
     if (lane == 0 && live) atomicAdd(&V.counters[0], 1ull);
+}
+
+// Log validation (csrc/mjx_validate.cuh): one warp = one whole log. The record is initialised in shared memory and never
+// written back; the only store is the 16-byte verdict.
+__global__ void __launch_bounds__(STEP_WARPS * 32) k_validate_logs(ValidateView V, Tables T, long long n_hdr) {
+    __shared__ __align__(16) unsigned char s_tab[STEP_WARPS][sizeof(TableState)];
+    __shared__ WarpScratch s_scratch[STEP_WARPS];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int i = blockIdx.x * STEP_WARPS + warp;
+    if (i >= V.n_logs) return;
+    const long long off = V.ev_off[i], cnt = V.ev_cnt[i];
+    if (off < 0 || cnt < 0 || off + cnt > n_hdr) {  // device-pointer callers: a log outside the word array is not read
+        if (lane == 0) V.out[i] = mjx_verdict{MJX_V_UNSUPPORTED, MJX_R_CAPACITY, 0, -1};
+        return;
+    }
+    constexpr int NV = sizeof(TableState) / 16;
+    uint4* dst = reinterpret_cast<uint4*>(s_tab[warp]);
+    for (int q = lane; q < NV; q += 32) dst[q] = make_uint4(0, 0, 0, 0);
+    __syncwarp();
+    Ctx c;
+    c.S = reinterpret_cast<TableState*>(s_tab[warp]);
+    c.W = &s_scratch[warp];
+    c.T = T;
+    c.lane = lane;
+    c.df = s_scratch[warp].dora_factor;
+    validate_log(c, V, i);
 }
 
 __global__ void k_begin_step(EnvView V) {
@@ -1106,6 +1133,65 @@ int mjx_env_create_replay(mjx_env** out, int n_jobs, const uint64_t* hdr, const 
     }();
     if (rc) return destroy_failed(out, env, rc);
     return MJX_OK;
+}
+
+// ---- bin/validate_logs.rs
+int mjx_validate_logs_dev(int n_logs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt, long long n_hdr,
+                          const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words, const uint64_t* hora_payload,
+                          const int32_t* hora_off, long long n_hora_words, mjx_verdict* out_verdicts, void* stream) {
+    if (!g_ready) return fail(MJX_ERR_STATE, "mjx_validate_logs: call mjx_init first");
+    if (n_logs <= 0 || !ev_off || !ev_cnt || !ky_off || !hora_off || !out_verdicts || n_hdr < 0 || (n_hdr > 0 && !hdr) ||
+        n_kyoku_words < 0 || n_kyoku_words % REPLAY_KYOKU_WORDS || (n_kyoku_words > 0 && !kyoku) || n_hora_words < 0 ||
+        n_hora_words % MJX_HORA_WORDS || (n_hora_words > 0 && !hora_payload))
+        return fail(MJX_ERR_ARG, "mjx_validate_logs: bad arguments");
+    ValidateView V;
+    V.hdr = hdr; V.ev_off = ev_off; V.ev_cnt = ev_cnt; V.kyoku = kyoku; V.ky_off = ky_off; V.hora = hora_payload; V.hora_off = hora_off;
+    V.n_kyoku = n_kyoku_words / REPLAY_KYOKU_WORDS; V.n_hora = n_hora_words / MJX_HORA_WORDS; V.n_logs = n_logs; V.out = out_verdicts;
+    k_validate_logs<<<(n_logs + STEP_WARPS - 1) / STEP_WARPS, STEP_WARPS * 32, 0, (cudaStream_t)stream>>>(V, g_T, n_hdr);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+int mjx_validate_logs(int n_logs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt, long long n_hdr,
+                      const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words, const uint64_t* hora_payload,
+                      const int32_t* hora_off, long long n_hora_words, mjx_verdict* out_verdicts, void* stream) {
+    if (!g_ready) return fail(MJX_ERR_STATE, "mjx_validate_logs: call mjx_init first");
+    if (n_logs <= 0 || !ev_off || !ev_cnt || !ky_off || !hora_off || !out_verdicts || n_hdr < 0 || (n_hdr > 0 && !hdr) ||
+        n_kyoku_words < 0 || n_kyoku_words % REPLAY_KYOKU_WORDS || (n_kyoku_words > 0 && !kyoku) || n_hora_words < 0 ||
+        n_hora_words % MJX_HORA_WORDS || (n_hora_words > 0 && !hora_payload))
+        return fail(MJX_ERR_ARG, "mjx_validate_logs: bad arguments");
+    for (int i = 0; i < n_logs; i++)
+        if (ev_off[i] < 0 || ev_cnt[i] < 0 || (long long)ev_off[i] + ev_cnt[i] > n_hdr || ky_off[i] < 0 || hora_off[i] < 0)
+            return fail(MJX_ERR_ARG, "mjx_validate_logs: log " + std::to_string(i) + " lies outside the arrays");
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t n = (size_t)n_logs, bh = sizeof(u64) * (size_t)n_hdr, bk = sizeof(u64) * (size_t)n_kyoku_words,
+                 bo = sizeof(u64) * (size_t)n_hora_words;
+    // one device allocation: words | payloads | hora entries | ev_off | ev_cnt | ky_off | hora_off | verdicts
+    const size_t total = bh + bk + bo + 4 * sizeof(i32) * n + sizeof(mjx_verdict) * n;
+    unsigned char* d = nullptr;
+    CU(cudaMalloc(&d, total));
+    u64* d_hdr = reinterpret_cast<u64*>(d);
+    u64* d_ky = reinterpret_cast<u64*>(d + bh);
+    u64* d_ho = reinterpret_cast<u64*>(d + bh + bk);
+    i32* d_i = reinterpret_cast<i32*>(d + bh + bk + bo);
+    mjx_verdict* d_out = reinterpret_cast<mjx_verdict*>(d_i + 4 * n);
+    int rc = [&]() -> int {
+        if (bh) CU(cudaMemcpyAsync(d_hdr, hdr, bh, cudaMemcpyHostToDevice, st));
+        if (bk) CU(cudaMemcpyAsync(d_ky, kyoku, bk, cudaMemcpyHostToDevice, st));
+        if (bo) CU(cudaMemcpyAsync(d_ho, hora_payload, bo, cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync(d_i, ev_off, sizeof(i32) * n, cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync(d_i + n, ev_cnt, sizeof(i32) * n, cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync(d_i + 2 * n, ky_off, sizeof(i32) * n, cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync(d_i + 3 * n, hora_off, sizeof(i32) * n, cudaMemcpyHostToDevice, st));
+        int r = mjx_validate_logs_dev(n_logs, bh ? d_hdr : nullptr, d_i, d_i + n, n_hdr, bk ? d_ky : nullptr, d_i + 2 * n, n_kyoku_words,
+                                      bo ? d_ho : nullptr, d_i + 3 * n, n_hora_words, d_out, stream);
+        if (r) return r;
+        CU(cudaMemcpyAsync(out_verdicts, d_out, sizeof(mjx_verdict) * n, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        return MJX_OK;
+    }();
+    cudaFree(d);
+    return rc;
 }
 
 // ---- libriichi.state.PlayerState batch

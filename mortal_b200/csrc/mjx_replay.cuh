@@ -48,6 +48,8 @@ MJX_D Reaction lw_reaction(u64 w, int type) {
 
 // PlayerState::update (state/update.rs:24-122) driven by one event word — for all four seats of a full-information record, or
 // for the single known seat of a PlayerState record (TableState.viewer1). `pay` = the start_kyoku payload (only read for that event).
+// KEEP_CANS = update_with_keep_cans(ev, true) (see ev_prologue).
+template <bool KEEP_CANS = false>
 MJX_DN void apply_event(Ctx& c, u64 w, const u64* pay, bool trust_seed) {
     TableState* S = c.S;
     switch (lw_type(w)) {
@@ -96,15 +98,16 @@ MJX_DN void apply_event(Ctx& c, u64 w, const u64* pay, bool trust_seed) {
         case LOG_ANKAN: ev_ankan(c, lw_reaction(w, R_ANKAN)); MJX_L0(S->kans += 1; S->bflags |= BF_DEAL_FROM_RINSHAN); break;
         case LOG_DORA:
             MJX_L0(if (S->n_dora < 5) S->wall[60 - S->n_dora] = (u8)lw_pai(w));
-            ev_dora(c);
+            ev_dora<KEEP_CANS>(c);
             break;
         case LOG_REACH: ev_reach(c, lw_actor(w)); break;
         case LOG_REACH_ACCEPTED:
             MJX_L0(S->riichi_to_be_accepted = (i8)lw_actor(w));
-            check_riichi_accepted(c);
+            check_riichi_accepted<KEEP_CANS>(c);
             break;
         default:  // start_game, hora, ryukyoku, end_kyoku, end_game: only the common prologue (update.rs:46-61)
-            ev_prologue(c, -1);
+            if (KEEP_CANS && lw_type(w) == LOG_HORA) ev_prologue<true>(c, -1);
+            else ev_prologue(c, -1);
             break;
     }
 }

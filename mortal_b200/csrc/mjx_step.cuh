@@ -250,13 +250,18 @@ MJX_DN bool ankan_after_riichi_ok(const Tables& T, const u8* tehai, int len_div3
 }
 
 // ---------------------------------------------------------------- event prologue (update.rs:46-61)
+// KEEP_CANS: update_with_keep_cans(ev, true) for an in-game announce (ReachAccepted / Dora / Hora): the seats keep their last
+// cans, target actor and kan candidates (only bin/validate_logs.rs asks for that; every other caller resets them).
+template <bool KEEP_CANS = false>
 MJX_D void ev_prologue(Ctx& c, int actor /* -1 if the event has no actor */) {
     MJX_FOR_SEATS(c, s) {
         SeatPrivate& P = c.S->priv[s];
-        P.cans = 0;
-        P.target_actor = (u8)(actor >= 0 ? actor : s);
-        P.ankan_cand = 0;
-        P.kakan_cand = 0;
+        if (!KEEP_CANS) {
+            P.cans = 0;
+            P.target_actor = (u8)(actor >= 0 ? actor : s);
+            P.ankan_cand = 0;
+            P.kakan_cand = 0;
+        }
         u16 f = P.flags;
         if (f & PF_MARK_SAME_CYCLE_FURITEN) f = (u16)((f & ~PF_MARK_SAME_CYCLE_FURITEN) | PF_AT_FURITEN);
         if (f & PF_CHANKAN_CHANCE) f = (u16)(f & ~(PF_CHANKAN_CHANCE | PF_AT_IPPATSU));
@@ -273,11 +278,12 @@ MJX_D void public_witness(TableState* S, int tile) {
 
 // ---------------------------------------------------------------- events
 // update.rs:780-808 + board.rs:353-364
+template <bool KEEP_CANS = false>
 MJX_D void ev_dora(Ctx& c) {
     TableState* S = c.S;
     if (S->n_dora >= 5) { set_err(c, ERR_FIFTH_KAN); return; }
     // ReachAccepted / Dora / Hora are "in-game announces" but the arena always resets cans (update.rs:25)
-    ev_prologue(c, -1);
+    ev_prologue<KEEP_CANS>(c, -1);
     MJX_L0(log_push(c, log_word(LOG_DORA, 0, 0, S->wall[60 - S->n_dora], 0, 0, 0, 0, 0, 0, 0));
            public_witness(S, S->wall[60 - S->n_dora]); S->n_dora += 1);
     recompute_dora_factor(c);
@@ -669,11 +675,12 @@ MJX_D void ev_reach(Ctx& c, int actor) {
 }
 
 // update.rs:677-686 + board.rs:342-351
+template <bool KEEP_CANS = false>
 MJX_D void check_riichi_accepted(Ctx& c) {
     TableState* S = c.S;
     if (S->riichi_to_be_accepted < 0) return;
     const int actor = S->riichi_to_be_accepted;
-    ev_prologue(c, actor);
+    ev_prologue<KEEP_CANS>(c, actor);
     MJX_L0(log_push(c, log_word(LOG_REACH_ACCEPTED, actor, 0, T_UNK, 0, 0, 0, 0, 0, 0, 0));
            S->riichi_to_be_accepted = -1;
            S->riichi_accepted |= (u8)(1 << actor);

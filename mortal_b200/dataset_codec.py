@@ -24,10 +24,26 @@ def _word(ty, actor=0, target=0, pai=37, tsumogiri=0, c=(0, 0, 0, 0)):
 KYOKU_WORDS = 19  # csrc/mjx_replay.cuh REPLAY_KYOKU_WORDS: 2 score words + the 136-byte wall (17 words)
 
 
-def encode_events(events, walls=None):
+HORA_WORDS = 2  # include/mjx.h MJX_HORA_WORDS
+
+
+def _hora_entry(ev, t):
+    """the facts of a hora the event word drops and bin/validate_logs.rs checks (include/mjx.h, mjx_validate_logs)"""
+    deltas, ura = ev.get("deltas"), ev.get("ura_markers")
+    w0 = (0 if deltas is None else int(deltas[ev["actor"]]) & 0xFFFFFFFF) | int(deltas is not None) << 32 | int(ura is not None) << 33
+    w1 = 0
+    if ura is not None:
+        w0 |= min(len(ura), 15) << 36
+        for k, x in enumerate(ura[:5]):
+            w1 |= t[x] << (8 * k)
+    return [w0, w1]
+
+
+def encode_events(events, walls=None, hora=None):
     """events: list of mjai dicts (a whole game, start_game .. end_game) -> (header words uint64 [n], kyoku payload uint64 [k, 19]).
     walls: optional uint8 [k, 136] (board.rs:109-122 layout) — the hidden tiles of every kyoku for the invisible observation;
-    without them only the 52 dealt tiles are known and the rest of the wall is `?`."""
+    without them only the 52 dealt tiles are known and the rest of the wall is `?`.
+    hora: optional list; every hora event appends its HORA_WORDS-word side entry (deltas[actor], ura markers) to it."""
     hdr, pay = [], []
     for ev in events:
         ty = _TYPES[ev["type"]]
@@ -61,9 +77,76 @@ def encode_events(events, walls=None):
             hdr.append(_word(ty, ev["actor"]))
         elif ty == HORA:
             hdr.append(_word(ty, ev["actor"], ev["target"]))
+            if hora is not None:
+                hora.append(_hora_entry(ev, t))
         else:  # ryukyoku, end_kyoku, start_game, end_game
             hdr.append(_word(ty))
     return np.array(hdr, dtype=np.uint64), np.array(pay, dtype=np.uint64).reshape(-1, KYOKU_WORDS)
+
+
+_ACTOR_FIELDS = {"tsumo": ("actor",), "dahai": ("actor",), "chi": ("actor", "target"), "pon": ("actor", "target"),
+                 "daiminkan": ("actor", "target"), "kakan": ("actor",), "ankan": ("actor",), "reach": ("actor",),
+                 "reach_accepted": ("actor",), "hora": ("actor", "target"), "start_kyoku": ("oya",)}
+_TILE_FIELDS = {"start_kyoku": ("bakaze", "dora_marker"), "tsumo": ("pai",), "dahai": ("pai",), "chi": ("pai",), "pon": ("pai",),
+                "daiminkan": ("pai",), "kakan": ("pai",), "dora": ("dora_marker",)}
+_CONSUMED = {"chi": 2, "pon": 2, "daiminkan": 3, "kakan": 3, "ankan": 4}
+
+
+def _is_int(x, lo, hi):
+    return isinstance(x, int) and not isinstance(x, bool) and lo <= x <= hi
+
+
+def check_event(ev):
+    """The structural checks deserialising an mjai Event makes (mjai/event.rs:20-120): None when `ev` is well formed, else the
+    name of the first failed check (the PARSE reasons of include/mjx.h). Unknown extra fields (such as `meta`) are ignored;
+    a missing `deltas` / `ura_markers` on a hora is not a parse error (bin/validate_logs.rs checks it)."""
+    if not isinstance(ev, dict):
+        return "json"
+    ty = ev.get("type")
+    if not isinstance(ty, str) or ty not in _TYPES:
+        return "unknown type"
+    for f in _ACTOR_FIELDS.get(ty, ()):
+        if f not in ev:
+            return "missing or invalid field"
+        if not _is_int(ev[f], 0, 3):
+            return "actor out of range"
+    for f in _TILE_FIELDS.get(ty, ()):
+        if f not in ev:
+            return "missing or invalid field"
+        if ev[f] not in TILE_ID:
+            return "unknown tile"
+    if ty in _CONSUMED:
+        c = ev.get("consumed")
+        if not isinstance(c, list):
+            return "missing or invalid field"
+        if len(c) != _CONSUMED[ty]:
+            return "consumed length"
+        if any(not isinstance(x, str) or x not in TILE_ID for x in c):
+            return "unknown tile"
+    if ty == "dahai" and not isinstance(ev.get("tsumogiri"), bool):
+        return "missing or invalid field"
+    if ty == "start_kyoku":
+        if not (_is_int(ev.get("kyoku"), 1, 4) and _is_int(ev.get("honba"), 0, 255) and _is_int(ev.get("kyotaku"), 0, 255)):
+            return "missing or invalid field"
+        sc = ev.get("scores")
+        if not (isinstance(sc, list) and len(sc) == 4 and all(_is_int(x, -2**31, 2**31 - 1) for x in sc)):
+            return "missing or invalid field"
+        th = ev.get("tehais")
+        if not (isinstance(th, list) and len(th) == 4 and all(isinstance(h, list) and len(h) == 13 for h in th)):
+            return "missing or invalid field"
+        if any(not isinstance(x, str) or x not in TILE_ID for h in th for x in h):
+            return "unknown tile"
+    if ty in ("hora", "ryukyoku") and ev.get("deltas") is not None:
+        d = ev["deltas"]
+        if not (isinstance(d, list) and len(d) == 4 and all(_is_int(x, -2**31, 2**31 - 1) for x in d)):
+            return "missing or invalid field"
+    if ty == "hora" and ev.get("ura_markers") is not None:
+        u = ev["ura_markers"]
+        if not isinstance(u, list):
+            return "missing or invalid field"
+        if any(not isinstance(x, str) or x not in TILE_ID for x in u):
+            return "unknown tile"
+    return None
 
 
 def _swap_tile(name: str) -> str:
