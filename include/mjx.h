@@ -187,6 +187,28 @@ int mjx_validate_logs_dev(int n_logs, const uint64_t* hdr, const int32_t* ev_off
                           const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words, const uint64_t* hora_payload,
                           const int32_t* hora_off, long long n_hora_words, mjx_verdict* out_verdicts, void* stream);
 
+/* ---- mjai log text -> event words on the device (csrc/mjx_mjai.cuh) -------------------------------------------------------
+ * `text`: every log's UTF-8 bytes, concatenated, log i = [log_off[i], log_off[i + 1]) (device arrays, log_off int64 [n_logs + 1]).
+ * A log is ACCEPTED when the decoder can show that Python's json reads it as the host path does (the rule is in
+ * csrc/mjx_mjai.cuh); an accepted log's arrays equal dataset_codec.encode_events over json.loads of its lines, in the
+ * mjx_validate_logs layout above (words, 19-word start_kyoku payloads, MJX_HORA_WORDS-word hora entries), plus the 1-based line
+ * number of every event. A DECLINED log is left to the host. `augment` != 0 applies Tile::augment (manzu <-> pinzu) to every
+ * tile as it is decoded. Two phases, both enqueued on `stream` without a synchronise:
+ *   mjx_mjai_count_dev  -> counts: device mjx_mjai_counts [n_logs] (a declined log: all zero, first_begin = first_end = -1);
+ *   mjx_mjai_fill_dev   the arrays of the accepted logs, log i's first word / line at ev_off[i], first payload at ky_off[i], first
+ *                       hora entry at hora_off[i] (device int32 [n_logs], typically exclusive sums of the counts copied to host);
+ *                       declined logs are skipped, and nothing is written past n_hdr / n_kyoku_words / n_hora_words. */
+typedef struct mjx_mjai_counts {
+    int32_t accept, n_events, n_kyoku, n_hora;
+    int32_t first_begin, first_end;  /* the first event line's bytes, relative to the log's start (start_game: names, seed) */
+} mjx_mjai_counts;
+int mjx_mjai_count_dev(int n_logs, const uint8_t* text, long long n_bytes, const int64_t* log_off, int augment,
+                       mjx_mjai_counts* counts, void* stream);
+int mjx_mjai_fill_dev(int n_logs, const uint8_t* text, long long n_bytes, const int64_t* log_off, int augment,
+                      const mjx_mjai_counts* counts, const int32_t* ev_off, const int32_t* ky_off, const int32_t* hora_off,
+                      uint64_t* hdr, int32_t* lines, long long n_hdr, uint64_t* kyoku, long long n_kyoku_words, uint64_t* hora_payload,
+                      long long n_hora_words, void* stream);
+
 /* ---- libriichi.state.PlayerState (state/player_state.rs:143-264, state/getter.rs:6-156, state/obs_repr.rs:776-791) ---------
  * A batch of n independent single-seat states: table records in single-seat mode (other seats' hidden tiles are `?` = 37), updated
  * by the same device event handlers self-play uses. `mjx_state_create` returns an mjx_env whose encoder entry points

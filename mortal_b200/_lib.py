@@ -99,6 +99,10 @@ SYMBOLS = {
                                     C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p]),
     "mjx_validate_logs_dev": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p,
                                         C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p]),
+    "mjx_mjai_count_dev": (C.c_int, [C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "mjx_mjai_fill_dev": (C.c_int, [C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p,
+                                    C.c_longlong, C.c_void_p]),
 }
 
 

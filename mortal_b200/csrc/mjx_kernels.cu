@@ -10,6 +10,7 @@
 #include "mjx_policy.cuh"
 #include "mjx_replay.cuh"
 #include "mjx_validate.cuh"
+#include "mjx_mjai.cuh"
 #include "mjx_invisible.cuh"
 #include "mjx_state.cuh"
 #include "mjx_nn.cuh"
@@ -106,6 +107,111 @@ __global__ void __launch_bounds__(STEP_WARPS * 32) k_validate_logs(ValidateView 
     c.lane = lane;
     c.df = s_scratch[warp].dora_factor;
     validate_log(c, V, i);
+}
+
+// mjai log text -> event words (csrc/mjx_mjai.cuh): one warp = one log. The warp reads the log in 128-byte steps, one byte per lane
+// and 32-byte window, queues the line ends the newline ballots find, and parses 32 queued lines at a time, one per lane. The count
+// pass writes mjx_mjai_counts; the fill pass repeats the walk over accepted logs and stores words, line numbers, start_kyoku
+// payloads and hora entries at the positions the caller derived from the counts (a start_kyoku or hora line is parsed a second
+// time to write its side data).
+constexpr int MJAI_WARPS = 4;
+struct MjaiView {
+    const u8* text;
+    long long n_bytes;
+    const i64* log_off;  // [n_logs + 1]
+    int n_logs, augment;
+    mjx_mjai_counts* counts;
+    const i32 *ev_off, *ky_off, *hora_off;  // fill pass
+    u64* hdr;
+    i32* lines;
+    u64 *kyoku, *hora;
+    long long n_hdr, n_kyoku, n_hora;  // capacities: words, payloads, entries
+};
+
+template <bool FILL>
+__global__ void __launch_bounds__(MJAI_WARPS * 32) k_mjai_decode(MjaiView V) {
+    __shared__ int s_end[MJAI_WARPS][64];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int i = blockIdx.x * MJAI_WARPS + warp;
+    if (i >= V.n_logs) return;
+    if (FILL && !V.counts[i].accept) return;
+    const long long lb = V.log_off[i], le = V.log_off[i + 1];
+    bool decline = lb < 0 || le <= lb || le > V.n_bytes || le - lb >= 0x7FFFFFFF;  // offsets within a log are int
+    const int len = decline ? 0 : (int)(le - lb);
+    const u8* p = V.text + (decline ? 0 : lb);
+    const bool aug = V.augment != 0;
+    const unsigned lt = (1u << lane) - 1;
+    int* q = s_end[warp];  // ends of the queued lines (the '\n', or len for a last line without one)
+    int qn = 0, start = 0, line_no = 0, n_ev = 0, n_ky = 0, n_ho = 0, first_b = -1, first_e = -1;
+    auto flush = [&](int cnt) {  // parses the first cnt (1..32) queued lines, lane j the j-th
+        // lanes >= cnt read stale queue entries for b / ce; they parse nothing and their values are never used
+        const int b = lane == 0 ? start : q[lane > 0 ? lane - 1 : 0] + 1;
+        int ce = lane < cnt ? q[lane] : b;
+        if (lane < cnt && ce < len && ce > b && p[ce - 1] == '\r') ce--;  // "\r\n"
+        MjaiLine ln{MJ_BLANK, 0, 0};
+        if (lane < cnt) ln = mjai_parse_line(p, b, ce, aug, nullptr, nullptr);
+        decline = decline || __any_sync(~0u, ln.kind == MJ_DECLINE);
+        if (!decline) {
+            const bool ev = ln.kind == MJ_EVENT;
+            const unsigned me = __ballot_sync(~0u, ev), mk = __ballot_sync(~0u, ev && ln.ty == MJT_START_KYOKU),
+                           mh = __ballot_sync(~0u, ev && ln.ty == MJT_HORA);
+            if (first_b < 0 && me) {
+                const int f = __ffs(me) - 1;
+                first_b = __shfl_sync(~0u, b, f);
+                first_e = __shfl_sync(~0u, ce, f);
+            }
+            if (FILL && ev) {
+                const long long at = (long long)V.ev_off[i] + n_ev + __popc(me & lt);
+                if (at >= 0 && at < V.n_hdr) { V.hdr[at] = ln.word; V.lines[at] = line_no + lane + 1; }
+                if (ln.ty == MJT_START_KYOKU) {
+                    const long long k = (long long)V.ky_off[i] + n_ky + __popc(mk & lt);
+                    if (k >= 0 && k < V.n_kyoku) mjai_parse_line(p, b, ce, aug, V.kyoku + k * MJAI_KYOKU_WORDS, nullptr);
+                } else if (ln.ty == MJT_HORA) {
+                    const long long k = (long long)V.hora_off[i] + n_ho + __popc(mh & lt);
+                    if (k >= 0 && k < V.n_hora) mjai_parse_line(p, b, ce, aug, nullptr, V.hora + k * MJX_HORA_WORDS);
+                }
+            }
+            n_ev += __popc(me); n_ky += __popc(mk); n_ho += __popc(mh);
+        }
+        line_no += cnt;
+        start = q[cnt - 1] + 1;
+        const int rest = qn - cnt, keep = lane < rest ? q[cnt + lane] : 0;
+        __syncwarp();
+        if (lane < rest) q[lane] = keep;
+        __syncwarp();
+        qn = rest;
+    };
+    for (int base = 0; base < len && !decline; base += 128) {
+        u8 x[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) x[k] = base + 32 * k + lane < len ? p[base + 32 * k + lane] : 0;
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            // qn < 32 here: a window adds at most 32 ends to the 64-entry queue, and a full queue is flushed at once. A decline
+            // (warp-uniform) ends the walk before anything more is queued.
+            if (decline) break;
+            const unsigned m = __ballot_sync(~0u, x[k] == '\n');
+            if (!m) continue;
+            if (x[k] == '\n') q[qn + __popc(m & lt)] = base + 32 * k + lane;
+            __syncwarp();
+            qn += __popc(m);
+            if (qn >= 32) flush(32);
+        }
+    }
+    if (!decline) {
+        const int next = qn ? q[qn - 1] + 1 : start;
+        __syncwarp();
+        if (next < len) {  // the last line has no line break
+            if (lane == 0) q[qn] = len;
+            __syncwarp();
+            qn++;
+        }
+        while (qn > 0 && !decline) flush(qn < 32 ? qn : 32);
+    }
+    if (!FILL && lane == 0) {
+        const bool ok = !decline && n_ev > 0;
+        V.counts[i] = mjx_mjai_counts{ok ? 1 : 0, ok ? n_ev : 0, ok ? n_ky : 0, ok ? n_ho : 0, ok ? first_b : -1, ok ? first_e : -1};
+    }
 }
 
 __global__ void k_begin_step(EnvView V) {
@@ -1192,6 +1298,37 @@ int mjx_validate_logs(int n_logs, const uint64_t* hdr, const int32_t* ev_off, co
     }();
     cudaFree(d);
     return rc;
+}
+
+// ---- mjai log text -> event words
+int mjx_mjai_count_dev(int n_logs, const uint8_t* text, long long n_bytes, const int64_t* log_off, int augment,
+                       mjx_mjai_counts* counts, void* stream) {
+    if (n_logs <= 0 || n_bytes < 0 || (n_bytes > 0 && !text) || !log_off || !counts)
+        return fail(MJX_ERR_ARG, "mjx_mjai_count_dev: bad arguments");
+    MjaiView V{};
+    V.text = text; V.n_bytes = n_bytes; V.log_off = log_off; V.n_logs = n_logs; V.augment = augment; V.counts = counts;
+    k_mjai_decode<false><<<(n_logs + MJAI_WARPS - 1) / MJAI_WARPS, MJAI_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+int mjx_mjai_fill_dev(int n_logs, const uint8_t* text, long long n_bytes, const int64_t* log_off, int augment,
+                      const mjx_mjai_counts* counts, const int32_t* ev_off, const int32_t* ky_off, const int32_t* hora_off,
+                      uint64_t* hdr, int32_t* lines, long long n_hdr, uint64_t* kyoku, long long n_kyoku_words, uint64_t* hora_payload,
+                      long long n_hora_words, void* stream) {
+    if (n_logs <= 0 || n_bytes < 0 || (n_bytes > 0 && !text) || !log_off || !counts || !ev_off || !ky_off || !hora_off ||
+        n_hdr < 0 || (n_hdr > 0 && (!hdr || !lines)) || n_kyoku_words < 0 || n_kyoku_words % REPLAY_KYOKU_WORDS ||
+        (n_kyoku_words > 0 && !kyoku) || n_hora_words < 0 || n_hora_words % MJX_HORA_WORDS || (n_hora_words > 0 && !hora_payload))
+        return fail(MJX_ERR_ARG, "mjx_mjai_fill_dev: bad arguments");
+    MjaiView V{};
+    V.text = text; V.n_bytes = n_bytes; V.log_off = log_off; V.n_logs = n_logs; V.augment = augment;
+    V.counts = const_cast<mjx_mjai_counts*>(counts);
+    V.ev_off = ev_off; V.ky_off = ky_off; V.hora_off = hora_off;
+    V.hdr = hdr; V.lines = lines; V.kyoku = kyoku; V.hora = hora_payload;
+    V.n_hdr = n_hdr; V.n_kyoku = n_kyoku_words / REPLAY_KYOKU_WORDS; V.n_hora = n_hora_words / MJX_HORA_WORDS;
+    k_mjai_decode<true><<<(n_logs + MJAI_WARPS - 1) / MJAI_WARPS, MJAI_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
+    CU(cudaGetLastError());
+    return MJX_OK;
 }
 
 // ---- libriichi.state.PlayerState batch
