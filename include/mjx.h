@@ -208,6 +208,44 @@ int mjx_mjai_fill_dev(int n_logs, const uint8_t* text, long long n_bytes, const 
                       const mjx_mjai_counts* counts, const int32_t* ev_off, const int32_t* ky_off, const int32_t* hora_off,
                       uint64_t* hdr, int32_t* lines, long long n_hdr, uint64_t* kyoku, long long n_kyoku_words, uint64_t* hora_payload,
                       long long n_hora_words, void* stream);
+/* mjx_mjai_fill_dev plus the per-event deltas array: everything mjx_mjai_fill_dev writes (bit-identical), and for every hora and
+ * ryukyoku event at word index e (= ev_off[i] + k):
+ *   deltas[4 * e + s] = the event's deltas[s] (int32; 0 when the field is absent or null),
+ *   has_deltas[e]     = 1 when `deltas` is present and not null, else 0.
+ * Both arrays have the word array's capacity n_hdr (deltas int32 [n_hdr, 4], has_deltas uint8 [n_hdr]); the entries of other
+ * events are not written. */
+int mjx_mjai_fill_deltas_dev(int n_logs, const uint8_t* text, long long n_bytes, const int64_t* log_off, int augment,
+                             const mjx_mjai_counts* counts, const int32_t* ev_off, const int32_t* ky_off, const int32_t* hora_off,
+                             uint64_t* hdr, int32_t* lines, long long n_hdr, uint64_t* kyoku, long long n_kyoku_words,
+                             uint64_t* hora_payload, long long n_hora_words, int32_t* deltas, uint8_t* has_deltas, void* stream);
+
+/* ---- per-player log statistics: stat.rs:263-442 Stat::from_game (csrc/mjx_stat.cuh) ------------------------------------------
+ * The counters of mortal_b200/stat.py Stat, in this order: X(name). This list is the single definition of the order (stat.py
+ * reads it); every counter is an int64. */
+#define MJX_STAT_COUNTERS(X)                                                                                                    \
+    X(game) X(round) X(oya) X(point) X(rank_1) X(rank_2) X(rank_3) X(rank_4) X(tobi)                                             \
+    X(agari) X(agari_as_oya) X(agari_jun) X(agari_point_oya) X(agari_point_ko)                                                  \
+    X(riichi) X(riichi_as_oya) X(riichi_jun) X(chasing_riichi) X(riichi_got_chased) X(riichi_agari) X(riichi_agari_jun)         \
+    X(riichi_agari_point) X(riichi_houjuu) X(riichi_ryukyoku) X(riichi_point)                                                   \
+    X(fuuro) X(fuuro_num) X(fuuro_agari) X(fuuro_agari_jun) X(fuuro_agari_point) X(fuuro_houjuu) X(fuuro_point)                 \
+    X(dama_agari) X(dama_agari_jun) X(dama_agari_point)                                                                         \
+    X(houjuu) X(houjuu_jun) X(houjuu_to_oya) X(houjuu_point_to_oya) X(houjuu_point_to_ko)                                       \
+    X(ryukyoku) X(ryukyoku_point) X(yakuman) X(nagashi_mangan)
+#define MJX_STAT_ENUM_(name) MJX_S_##name,
+enum mjx_stat_counter { MJX_STAT_COUNTERS(MJX_STAT_ENUM_) MJX_STAT_N };
+#undef MJX_STAT_ENUM_
+/* The per-log status: OK = counted; otherwise the log's counters are all zero and the caller decides (mortal_b200/stat.py reads
+ * such a log on the host). NO_DELTAS: a seat is selected and a hora or ryukyoku has no usable deltas; CAPACITY: the log's
+ * events or start_kyoku payloads lie outside the arrays. */
+enum mjx_stat_status { MJX_STAT_OK = 0, MJX_STAT_NOT_START_GAME = 1, MJX_STAT_NO_DELTAS = 2, MJX_STAT_CAPACITY = 3 };
+/* Stat.from_game summed over the selected seats of every log, over the arrays of mjx_mjai_fill_deltas_dev (device pointers):
+ * event words hdr [n_hdr] with ev_off / ev_cnt [n_logs]; start_kyoku payloads kyoku [n_kyoku_words] (19 words each, log i's first
+ * at ky_off[i]; the scores are words 0-1); deltas / has_deltas [n_hdr] as above; seats uint8 [n_logs] (bit s: take seat s's
+ * stats). out: int64 [n_logs, MJX_STAT_N] (`game` counts once per selected seat); status: int32 [n_logs] mjx_stat_status.
+ * One warp per log; enqueued on `stream` without a synchronise. Every read is bounded by n_hdr / n_kyoku_words. */
+int mjx_stat_logs_dev(int n_logs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt, long long n_hdr,
+                      const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words, const int32_t* deltas,
+                      const uint8_t* has_deltas, const uint8_t* seats, int64_t* out, int32_t* status, void* stream);
 
 /* ---- libriichi.state.PlayerState (state/player_state.rs:143-264, state/getter.rs:6-156, state/obs_repr.rs:776-791) ---------
  * A batch of n independent single-seat states: table records in single-seat mode (other seats' hidden tiles are `?` = 37), updated

@@ -103,6 +103,11 @@ SYMBOLS = {
     "mjx_mjai_fill_dev": (C.c_int, [C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p,
                                     C.c_longlong, C.c_void_p]),
+    "mjx_mjai_fill_deltas_dev": (C.c_int, [C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong,
+                                           C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mjx_stat_logs_dev": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong,
+                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 

@@ -11,6 +11,7 @@
 #include "mjx_replay.cuh"
 #include "mjx_validate.cuh"
 #include "mjx_mjai.cuh"
+#include "mjx_stat.cuh"
 #include "mjx_invisible.cuh"
 #include "mjx_state.cuh"
 #include "mjx_nn.cuh"
@@ -113,7 +114,8 @@ __global__ void __launch_bounds__(STEP_WARPS * 32) k_validate_logs(ValidateView 
 // and 32-byte window, queues the line ends the newline ballots find, and parses 32 queued lines at a time, one per lane. The count
 // pass writes mjx_mjai_counts; the fill pass repeats the walk over accepted logs and stores words, line numbers, start_kyoku
 // payloads and hora entries at the positions the caller derived from the counts (a start_kyoku or hora line is parsed a second
-// time to write its side data).
+// time to write its side data). The DELTAS fill also stores every hora's and ryukyoku's four deltas at the event's index, parsing
+// that line a second time.
 constexpr int MJAI_WARPS = 4;
 struct MjaiView {
     const u8* text;
@@ -127,9 +129,13 @@ struct MjaiView {
     u64 *kyoku, *hora;
     long long n_hdr, n_kyoku, n_hora;  // capacities: words, payloads, entries
 };
+struct MjaiDeltas {  // the DELTAS fill's outputs, capacity n_hdr (a separate parameter: the other passes never capture it)
+    i32* deltas;     // [n_hdr, 4]
+    u8* has_deltas;  // [n_hdr]
+};
 
-template <bool FILL>
-__global__ void __launch_bounds__(MJAI_WARPS * 32) k_mjai_decode(MjaiView V) {
+template <bool FILL, bool DELTAS>
+__global__ void __launch_bounds__(MJAI_WARPS * 32) k_mjai_decode(MjaiView V, MjaiDeltas Dl) {
     __shared__ int s_end[MJAI_WARPS][64];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int i = blockIdx.x * MJAI_WARPS + warp;
@@ -163,6 +169,13 @@ __global__ void __launch_bounds__(MJAI_WARPS * 32) k_mjai_decode(MjaiView V) {
             if (FILL && ev) {
                 const long long at = (long long)V.ev_off[i] + n_ev + __popc(me & lt);
                 if (at >= 0 && at < V.n_hdr) { V.hdr[at] = ln.word; V.lines[at] = line_no + lane + 1; }
+                if constexpr (DELTAS) {
+                    if ((ln.ty == MJT_HORA || ln.ty == MJT_RYUKYOKU) && at >= 0 && at < V.n_hdr) {
+                        i32 d[4];
+                        Dl.has_deltas[at] = mjai_line_deltas(p, b, ce, d) ? 1 : 0;
+                        reinterpret_cast<int4*>(Dl.deltas)[at] = make_int4(d[0], d[1], d[2], d[3]);
+                    }
+                }
                 if (ln.ty == MJT_START_KYOKU) {
                     const long long k = (long long)V.ky_off[i] + n_ky + __popc(mk & lt);
                     if (k >= 0 && k < V.n_kyoku) mjai_parse_line(p, b, ce, aug, V.kyoku + k * MJAI_KYOKU_WORDS, nullptr);
@@ -212,6 +225,23 @@ __global__ void __launch_bounds__(MJAI_WARPS * 32) k_mjai_decode(MjaiView V) {
         const bool ok = !decline && n_ev > 0;
         V.counts[i] = mjx_mjai_counts{ok ? 1 : 0, ok ? n_ev : 0, ok ? n_ky : 0, ok ? n_ho : 0, ok ? first_b : -1, ok ? first_e : -1};
     }
+}
+
+// Per-player statistics (csrc/mjx_stat.cuh): one warp = one log. Lanes 0..3 keep seats 0..3's counters in shared memory; the warp
+// loads the event words 32 at a time (coalesced) and shuffles each word to the seat lanes.
+__global__ void __launch_bounds__(STAT_WARPS * 32) k_stat_logs(StatView V) {
+    __shared__ i64 s_c[STAT_WARPS][4][MJX_STAT_N];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int i = blockIdx.x * STAT_WARPS + warp;
+    if (i >= V.n_logs) return;
+    i64(*c)[MJX_STAT_N] = s_c[warp];
+    for (int k = lane; k < 4 * MJX_STAT_N; k += 32) c[k / MJX_STAT_N][k % MJX_STAT_N] = 0;
+    __syncwarp();
+    const int status = stat_log(V, i, lane, c);
+    __syncwarp();
+    for (int k = lane; k < MJX_STAT_N; k += 32)
+        V.out[(long long)i * MJX_STAT_N + k] = status ? 0 : c[0][k] + c[1][k] + c[2][k] + c[3][k];
+    if (lane == 0) V.status[i] = status;
 }
 
 __global__ void k_begin_step(EnvView V) {
@@ -1307,7 +1337,7 @@ int mjx_mjai_count_dev(int n_logs, const uint8_t* text, long long n_bytes, const
         return fail(MJX_ERR_ARG, "mjx_mjai_count_dev: bad arguments");
     MjaiView V{};
     V.text = text; V.n_bytes = n_bytes; V.log_off = log_off; V.n_logs = n_logs; V.augment = augment; V.counts = counts;
-    k_mjai_decode<false><<<(n_logs + MJAI_WARPS - 1) / MJAI_WARPS, MJAI_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
+    k_mjai_decode<false, false><<<(n_logs + MJAI_WARPS - 1) / MJAI_WARPS, MJAI_WARPS * 32, 0, (cudaStream_t)stream>>>(V, MjaiDeltas{});
     CU(cudaGetLastError());
     return MJX_OK;
 }
@@ -1326,7 +1356,45 @@ int mjx_mjai_fill_dev(int n_logs, const uint8_t* text, long long n_bytes, const 
     V.ev_off = ev_off; V.ky_off = ky_off; V.hora_off = hora_off;
     V.hdr = hdr; V.lines = lines; V.kyoku = kyoku; V.hora = hora_payload;
     V.n_hdr = n_hdr; V.n_kyoku = n_kyoku_words / REPLAY_KYOKU_WORDS; V.n_hora = n_hora_words / MJX_HORA_WORDS;
-    k_mjai_decode<true><<<(n_logs + MJAI_WARPS - 1) / MJAI_WARPS, MJAI_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
+    k_mjai_decode<true, false><<<(n_logs + MJAI_WARPS - 1) / MJAI_WARPS, MJAI_WARPS * 32, 0, (cudaStream_t)stream>>>(V, MjaiDeltas{});
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+int mjx_mjai_fill_deltas_dev(int n_logs, const uint8_t* text, long long n_bytes, const int64_t* log_off, int augment,
+                             const mjx_mjai_counts* counts, const int32_t* ev_off, const int32_t* ky_off, const int32_t* hora_off,
+                             uint64_t* hdr, int32_t* lines, long long n_hdr, uint64_t* kyoku, long long n_kyoku_words,
+                             uint64_t* hora_payload, long long n_hora_words, int32_t* deltas, uint8_t* has_deltas, void* stream) {
+    if (n_logs <= 0 || n_bytes < 0 || (n_bytes > 0 && !text) || !log_off || !counts || !ev_off || !ky_off || !hora_off ||
+        n_hdr < 0 || (n_hdr > 0 && (!hdr || !lines || !deltas || !has_deltas)) || ((uintptr_t)deltas & 15) ||
+        n_kyoku_words < 0 || n_kyoku_words % REPLAY_KYOKU_WORDS || (n_kyoku_words > 0 && !kyoku) || n_hora_words < 0 ||
+        n_hora_words % MJX_HORA_WORDS || (n_hora_words > 0 && !hora_payload))
+        return fail(MJX_ERR_ARG, "mjx_mjai_fill_deltas_dev: bad arguments");
+    MjaiView V{};
+    V.text = text; V.n_bytes = n_bytes; V.log_off = log_off; V.n_logs = n_logs; V.augment = augment;
+    V.counts = const_cast<mjx_mjai_counts*>(counts);
+    V.ev_off = ev_off; V.ky_off = ky_off; V.hora_off = hora_off;
+    V.hdr = hdr; V.lines = lines; V.kyoku = kyoku; V.hora = hora_payload;
+    V.n_hdr = n_hdr; V.n_kyoku = n_kyoku_words / REPLAY_KYOKU_WORDS; V.n_hora = n_hora_words / MJX_HORA_WORDS;
+    k_mjai_decode<true, true><<<(n_logs + MJAI_WARPS - 1) / MJAI_WARPS, MJAI_WARPS * 32, 0, (cudaStream_t)stream>>>(
+        V, MjaiDeltas{deltas, has_deltas});
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+// ---- per-player log statistics (stat.rs Stat::from_game)
+int mjx_stat_logs_dev(int n_logs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt, long long n_hdr,
+                      const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words, const int32_t* deltas,
+                      const uint8_t* has_deltas, const uint8_t* seats, int64_t* out, int32_t* status, void* stream) {
+    if (n_logs <= 0 || !ev_off || !ev_cnt || !ky_off || !seats || !out || !status || n_hdr < 0 ||
+        (n_hdr > 0 && (!hdr || !deltas || !has_deltas)) || n_kyoku_words < 0 || n_kyoku_words % REPLAY_KYOKU_WORDS ||
+        (n_kyoku_words > 0 && !kyoku))
+        return fail(MJX_ERR_ARG, "mjx_stat_logs_dev: bad arguments");
+    StatView V;
+    V.hdr = hdr; V.ev_off = ev_off; V.ev_cnt = ev_cnt; V.n_hdr = n_hdr; V.kyoku = kyoku; V.ky_off = ky_off;
+    V.n_kyoku = n_kyoku_words / REPLAY_KYOKU_WORDS; V.deltas = deltas; V.has_deltas = has_deltas; V.seats = seats; V.n_logs = n_logs;
+    V.out = out; V.status = status;
+    k_stat_logs<<<(n_logs + STAT_WARPS - 1) / STAT_WARPS, STAT_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
     CU(cudaGetLastError());
     return MJX_OK;
 }

@@ -454,4 +454,32 @@ MJX_DN MjaiLine mjai_parse_line(const u8* p, long long b, long long e, bool aug,
     return L;
 }
 
+// The `deltas` of a line mjai_parse_line accepted as a hora or ryukyoku -> d[0..4) (zeros when absent or null); true when the
+// field is present and not null. The line is known to be well formed, so the walk only looks for the key (given once, unescaped).
+MJX_DN bool mjai_line_deltas(const u8* p, long long b, long long e, i32* d) {
+    for (int k = 0; k < 4; k++) d[k] = 0;
+    MjCur c{p, b, e};
+    mj_ws(c);
+    if (mj_peek(c) != '{') return false;
+    c.i++;
+    mj_ws(c);
+    while (mj_peek(c) == '"') {
+        long long kb, ke, v[4];
+        bool esc;
+        if (!mj_key(c, &kb, &ke, &esc)) return false;
+        const long long v0 = c.i;
+        if (!mj_skip(c)) return false;
+        if (!esc && mj_eq(p, kb, ke, "deltas")) {
+            if (mj_is_null(p, v0, c.i) || !mj_ints(p, v0, c.i, 4, -2147483648LL, 2147483647LL, v)) return false;
+            for (int k = 0; k < 4; k++) d[k] = (i32)v[k];
+            return true;
+        }
+        mj_ws(c);
+        if (mj_peek(c) != ',') return false;
+        c.i++;
+        mj_ws(c);
+    }
+    return false;
+}
+
 }  // namespace mjx

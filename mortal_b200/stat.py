@@ -1,14 +1,29 @@
 """libriichi.stat.Stat — per-player statistics over mjai logs (stat.rs:26-124 fields, 263-442 accumulation, 447-515 loaders,
-516-786 derived rates). Host-side log arithmetic, no device work; used by mortal/player.py:71 and the test-play report of
-mortal/train.py:321-350. Counters are plain integer attributes with the reference's names; every derived quantity is a
-property `numerator / denominator` in float64 with IEEE semantics (0/0 = nan, x/0 = ±inf) like the Rust `as f64` divisions.
+516-786 derived rates); used by mortal/player.py:71 and the test-play report of mortal/train.py:321-350. Counters are plain
+integer attributes with the reference's names; every derived quantity is a property `numerator / denominator` in float64 with
+IEEE semantics (0/0 = nan, x/0 = ±inf) like the Rust `as f64` divisions.
+
+    Stat.from_dir(dir, player_name)            (every dir/**/*.json and dir/**/*.json.gz)
+    python -m mortal_b200.stat DIR PLAYER_NAME (bin/stat.rs: prints the reference's report)
+
+With libmjx built and a CUDA device present, from_dir decodes the log texts on the device (k_mjai_decode with the deltas output,
+csrc/mjx_mjai.cuh) and runs Stat.from_game there for every selected seat (k_stat_logs, csrc/mjx_stat.cuh); the counters are
+summed on the device and copied back once per chunk. A file the device cannot take as it is (unreadable, not gzip, not UTF-8,
+declined by the decoder, a hora or ryukyoku without deltas for a selected seat, a first event that is not start_game, a selected
+seat past 3) is read by the host code below, so it gives the same counters or raises the same exception. Without the library or
+a device, every file is read on the host.
 """
 from __future__ import annotations
 
 import glob
 import gzip
 import json
+import locale
+import math
 import os
+import re
+import sys
+from concurrent.futures import ThreadPoolExecutor
 
 COUNTERS = (
     "game round oya point rank_1 rank_2 rank_3 rank_4 tobi "
@@ -50,6 +65,11 @@ RATES = {
     "houjuu_rate_after_fuuro": ("fuuro_houjuu", "fuuro"), "avg_fuuro_point": ("fuuro_point", "fuuro"),
     "yakuman_rate": ("yakuman", "round"), "nagashi_mangan_rate": ("nagashi_mangan", "round"),
 }
+# from_dir's device path decodes and counts the files in chunks of consecutive files: at most CHUNK_LOGS files and, unless a
+# single file is larger, CHUNK_BYTES of decompressed text. The text of a chunk is held three times (the file contents, the pinned
+# staging buffer, the device copy), so this bounds memory whatever the corpus size.
+CHUNK_LOGS = 4096
+CHUNK_BYTES = 256 << 20
 
 
 def _fdiv(a: float, b: float) -> float:
@@ -183,17 +203,12 @@ class Stat:
 
     @staticmethod
     def from_dir(dir: str, player_name: str, disable_progress_bar: bool = False) -> "Stat":
+        paths = _log_paths(dir)
+        if _device_ready():
+            return _device_from_dir(paths, player_name)
         total = Stat()
-        paths = glob.glob(os.path.join(dir, "**", "*.json"), recursive=True) + glob.glob(os.path.join(dir, "**", "*.json.gz"), recursive=True)
         for path in paths:
-            opener = gzip.open if path.lower().endswith(".gz") else open
-            with opener(path, "rt") as f:
-                events = [json.loads(ln) for ln in f if ln.strip()]
-            if not events or events[0].get("type") != "start_game":
-                raise ValueError(f"first event is not start_game, got {events[0] if events else None!r}")
-            for i, name in enumerate(events[0].get("names", [])):
-                if name == player_name:
-                    total = total + Stat.from_game(events, i)
+            total = total + _host_log_stat(path, player_name)
         return total
 
     def __repr__(self):
@@ -208,3 +223,224 @@ class Stat:
                   f"Total score delta {self.point}", ""]
         lines += [f"{name} {getattr(self, name):.6f}" for name in RATES if not name.startswith("rank_") and name != "tobi_rate"]
         return "\n".join(lines)
+
+    def reference_text(self) -> str:
+        """the reference's report (the Display format of stat.rs:128-189): labels padded per block, Rust float formatting"""
+        pt = [90, 45, 0, -135]
+        blocks = [
+            [("Games", self.game), ("Rounds", self.round), ("Rounds as dealer", self.oya)],
+            [(f"{k}{('st', 'nd', 'rd', 'th')[k - 1]} (rate)", f"{getattr(self, f'rank_{k}')} ({_rs(getattr(self, f'rank_{k}_rate'))})")
+             for k in (1, 2, 3, 4)]
+            + [("Tobi(rate)", f"{self.tobi} ({_rs(self.tobi_rate)})"), ("Avg rank", _rs(self.avg_rank)),
+               ("Total rank pt", self.total_pt(pt)), ("Avg rank pt", _rs(self.avg_pt(pt))), ("Total Δscore", self.point),
+               ("Avg game Δscore", _rs(self.avg_point_per_game)), ("Avg round Δscore", _rs(self.avg_point_per_round))],
+        ]
+        blocks += [[(label, _rs(getattr(self, rate))) for label, rate in block] for block in _REFERENCE_RATES]
+        blocks.append([("Yakuman (rate)", f"{self.yakuman} ({_rs(self.yakuman_rate, 9)})"),
+                       ("Nagashi mangan (rate)", f"{self.nagashi_mangan} ({_rs(self.nagashi_mangan_rate, 9)})")])
+        out = []
+        for block in blocks:
+            w = max(len(label) for label, _ in block)
+            out.append("\n".join(f"{label.ljust(w)} {value}" for label, value in block))
+        return "\n\n".join(out)
+
+
+# the rate blocks of the reference's report (stat.rs:128-189), label -> derived quantity
+_REFERENCE_RATES = (
+    (("Win rate", "agari_rate"), ("Deal-in rate", "houjuu_rate"), ("Call rate", "fuuro_rate"), ("Riichi rate", "riichi_rate"),
+     ("Ryukyoku rate", "ryukyoku_rate")),
+    (("Avg winning Δscore", "avg_point_per_agari"), ("Avg winning Δscore as dealer", "avg_point_per_oya_agari"),
+     ("Avg winning Δscore as non-dealer", "avg_point_per_ko_agari"),
+     ("Avg riichi winning Δscore", "avg_point_per_riichi_agari"), ("Avg open winning Δscore", "avg_point_per_fuuro_agari"),
+     ("Avg dama winning Δscore", "avg_point_per_dama_agari"), ("Avg ryukyoku Δscore", "avg_point_per_ryukyoku")),
+    (("Avg winning turn", "avg_agari_jun"), ("Avg riichi winning turn", "avg_riichi_agari_jun"),
+     ("Avg open winning turn", "avg_fuuro_agari_jun"), ("Avg dama winning turn", "avg_dama_agari_jun")),
+    (("Avg deal-in turn", "avg_houjuu_jun"), ("Avg deal-in Δscore", "avg_point_per_houjuu"),
+     ("Avg deal-in Δscore to dealer", "avg_point_per_houjuu_to_oya"),
+     ("Avg deal-in Δscore to non-dealer", "avg_point_per_houjuu_to_ko")),
+    (("Chasing riichi rate", "chasing_riichi_rate"), ("Riichi chased rate", "riichi_chased_rate"),
+     ("Winning rate after riichi", "agari_rate_after_riichi"), ("Deal-in rate after riichi", "houjuu_rate_after_riichi"),
+     ("Avg riichi turn", "avg_riichi_jun"), ("Avg riichi Δscore", "avg_riichi_point")),
+    (("Avg number of calls", "avg_fuuro_num"), ("Winning rate after call", "agari_rate_after_fuuro"),
+     ("Deal-in rate after call", "houjuu_rate_after_fuuro"), ("Avg call Δscore", "avg_fuuro_point")),
+    (("Dealer wins/all dealer rounds", "agari_rate_as_oya"), ("Dealer wins/all wins", "agari_as_oya_rate"),
+     ("Deal-in to dealer/all deal-ins", "houjuu_to_oya_rate")),
+)
+
+
+def _rs(x: float, prec: int = 6) -> str:
+    """Rust's `{:.prec}` of an f64: Python's fixed-point digits, but `NaN`, `inf` and `-inf` for the non-finite values"""
+    if math.isnan(x):
+        return "NaN"
+    if math.isinf(x):
+        return "inf" if x > 0 else "-inf"
+    return f"{x:.{prec}f}"
+
+
+def _log_paths(dir: str):
+    return glob.glob(os.path.join(dir, "**", "*.json"), recursive=True) + glob.glob(os.path.join(dir, "**", "*.json.gz"), recursive=True)
+
+
+def _host_log_stat(path: str, player_name: str) -> Stat:
+    """one log file on the host: json.loads of every line, then Stat.from_game for every seat named player_name"""
+    opener = gzip.open if path.lower().endswith(".gz") else open
+    with opener(path, "rt") as f:
+        events = [json.loads(ln) for ln in f if ln.strip()]
+    if not events or events[0].get("type") != "start_game":
+        raise ValueError(f"first event is not start_game, got {events[0] if events else None!r}")
+    total = Stat()
+    for i, name in enumerate(events[0].get("names", [])):
+        if name == player_name:
+            total = total + Stat.from_game(events, i)
+    return total
+
+
+def _read_counters():
+    """the counter names of include/mjx.h MJX_STAT_COUNTERS, in the order k_stat_logs writes them (the header is their single
+    definition)"""
+    from . import _lib
+
+    with open(os.path.join(os.path.dirname(_lib.HERE), "include", "mjx.h")) as f:
+        text = f.read()
+    block = text[text.index("#define MJX_STAT_COUNTERS(X)"):]
+    block = block[:block.index("#define MJX_STAT_ENUM_")]
+    return tuple(re.findall(r"X\((\w+)\)", block))
+
+
+def _device_ready() -> bool:
+    """the device path needs the built library, a CUDA device, and a UTF-8 locale (the host path reads the files in the locale's
+    encoding; the decoder reads UTF-8)"""
+    from . import _lib
+
+    if not os.path.exists(_lib.lib_path()) or locale.getpreferredencoding(False).lower().replace("-", "") != "utf8":
+        return False
+    try:
+        import torch
+    except ImportError:
+        return False
+    return torch.cuda.is_available()
+
+
+def _read_bytes(path: str):
+    """a file's bytes, gunzipped for `.gz`; None when that fails (the host path then decides)"""
+    try:
+        if path.lower().endswith(".gz"):
+            with gzip.open(path, "rb") as f:
+                return f.read()
+        with open(path, "rb") as f:
+            return f.read()
+    except Exception:  # noqa: BLE001 — any failure: the host path raises its own exception for this file
+        return None
+
+
+def _seat_mask(blob: bytes, b: int, e: int, player_name: str):
+    """the seats named player_name on a log's first event line (bytes [b, e)) as a bit mask, or None when the host must decide"""
+    try:
+        first = json.loads(blob[b:e].decode("utf-8"))
+        if first.get("type") != "start_game":
+            return None
+        seats = [i for i, name in enumerate(first.get("names", [])) if name == player_name]
+    except Exception:  # noqa: BLE001
+        return None
+    if any(i > 3 for i in seats):
+        return None
+    return sum(1 << i for i in seats)
+
+
+def _stat_device() -> int:
+    """the GPU from_dir runs on: the one libmjx is initialised on (the library serves one device per process, so a process whose
+    arena or engine lives on cuda:k counts there too), else torch's current device"""
+    from . import _lib
+
+    if _lib._INIT_DEVICE is not None:
+        return _lib._INIT_DEVICE
+    import torch
+
+    return torch.cuda.current_device()
+
+
+def _chunks(paths, pool, step: int):
+    """(paths, contents) of consecutive files in order, read + gunzipped on `pool` `step` at a time, cut at CHUNK_LOGS files or
+    CHUNK_BYTES of text (a chunk always takes at least one file)"""
+    cur, size, lo = [], 0, 0
+    for s in range(0, len(paths), step):
+        for b in pool.map(_read_bytes, paths[s:s + step]):
+            n = len(b) if b is not None else 0
+            if cur and (len(cur) >= CHUNK_LOGS or size + n > CHUNK_BYTES):
+                yield paths[lo:lo + len(cur)], cur
+                lo += len(cur); cur, size = [], 0
+            cur.append(b); size += n
+    if cur:
+        yield paths[lo:lo + len(cur)], cur
+
+
+def _device_from_dir(paths, player_name: str, device: int | None = None) -> Stat:
+    """from_dir on the device (default: _stat_device()): per chunk of files, read + gunzip on a thread pool, decode with the deltas
+    output, k_stat_logs over the seats of every log, the counters summed on the device and copied back once; the rest of the
+    chunk's files, in glob order, through _host_log_stat"""
+    import numpy as np
+    import torch
+
+    from . import _lib
+    from .validate_logs import decode_dev
+
+    device = _stat_device() if device is None else device
+    _lib.init(device)
+    L = _lib.load()
+    dev = torch.device("cuda", device)
+    names = _read_counters()
+    total = {c: 0 for c in COUNTERS}
+    host_total = Stat()
+    workers = min(32, os.cpu_count() or 1)
+    # torch.cuda.device: the streams and allocations below belong to `device` whatever torch's current device is
+    with torch.cuda.device(device), ThreadPoolExecutor(workers) as pool:  # zlib and file reads release the GIL
+        for chunk, blobs in _chunks(paths, pool, 4 * workers):
+            on_dev = [k for k, b in enumerate(blobs) if b is not None]
+            host = [k for k, b in enumerate(blobs) if b is None]
+            if on_dev:
+                D = decode_dev([blobs[k] for k in on_dev], device, deltas=True)
+                seats = np.zeros(len(on_dev), dtype=np.uint8)
+                counted = []
+                for j, k in enumerate(on_dev):
+                    m = _seat_mask(blobs[k], int(D.counts[j, 4]), int(D.counts[j, 5]), player_name) if D.accept[j] else None
+                    if m is None:
+                        host.append(k)
+                    else:
+                        seats[j] = m; counted.append(j)
+                n = len(on_dev)
+                out = torch.empty((n, len(names)), dtype=torch.int64, device=dev)
+                status = torch.empty(n, dtype=torch.int32, device=dev)
+                d_seats = torch.from_numpy(seats).to(dev)
+                ptr = lambda t: t.data_ptr() if t.numel() else None
+                _lib.check(L.mjx_stat_logs_dev(n, ptr(D.hdr), D.offs[0].data_ptr(), D.offs[1].data_ptr(), D.hdr.numel(),
+                                               ptr(D.kyoku), D.offs[2].data_ptr(), D.kyoku.numel(), ptr(D.deltas), ptr(D.has_deltas),
+                                               d_seats.data_ptr(), out.data_ptr(), status.data_ptr(),
+                                               torch.cuda.current_stream(dev).cuda_stream), "mjx_stat_logs_dev")
+                # a log with a non-zero status has all-zero counters, so the sum counts exactly the logs with status 0
+                res = torch.cat([out.sum(0), status.to(torch.int64)]).cpu().numpy()
+                for name, v in zip(names, res[:len(names)]):
+                    total[name] += int(v)
+                st = res[len(names):]
+                host += [on_dev[j] for j in counted if st[j] != 0]
+            for k in sorted(host):
+                host_total = host_total + _host_log_stat(chunk[k], player_name)
+    return Stat(**total) + host_total
+
+
+def main(argv=None) -> int:
+    """bin/stat.rs: the report of Stat.from_dir(DIR, PLAYER_NAME) on stdout"""
+    argv = sys.argv[1:] if argv is None else argv
+    if len(argv) != 2:
+        print("Usage: python -m mortal_b200.stat <DIR> <PLAYER_NAME>", file=sys.stderr)
+        return 2
+    try:
+        st = Stat.from_dir(argv[0], argv[1], disable_progress_bar=True)
+    except Exception as e:  # noqa: BLE001 — the reference's `Error: ...` exit
+        print(f"Error: {type(e).__name__}: {e}", file=sys.stderr)
+        return 1
+    print(st.reference_text())
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

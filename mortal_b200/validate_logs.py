@@ -126,10 +126,13 @@ class DecodedLogs:
     lines: object       # int32 [n_events] device: 1-based line of every event
     kyoku: object       # int64 [n_kyoku * KYOKU_WORDS] device
     hora: object        # int64 [n_hora * HORA_WORDS] device
+    deltas: object = None      # with deltas=True: int32 [n_events, 4] device, every hora's and ryukyoku's deltas at its event
+    has_deltas: object = None  # with deltas=True: uint8 [n_events] device, 1 where that event's `deltas` is present and not null
 
 
-def decode_dev(blobs, device: int = 0, augment: bool = False) -> DecodedLogs:
-    """UTF-8 log texts (bytes) -> DecodedLogs, decoded on `device` (csrc/mjx_mjai.cuh); the one device-to-host copy is the counts"""
+def decode_dev(blobs, device: int = 0, augment: bool = False, deltas: bool = False) -> DecodedLogs:
+    """UTF-8 log texts (bytes) -> DecodedLogs, decoded on `device` (csrc/mjx_mjai.cuh); the one device-to-host copy is the counts.
+    `deltas` also fills the per-event deltas arrays (mjx_mjai_fill_deltas_dev); the other arrays are the same either way."""
     import torch
 
     L = _lib.load()
@@ -159,6 +162,15 @@ def decode_dev(blobs, device: int = 0, augment: bool = False) -> DecodedLogs:
     kyoku = torch.empty(n_k * KYOKU_WORDS, dtype=torch.int64, device=dev)
     hora = torch.empty(n_h * HORA_WORDS, dtype=torch.int64, device=dev)
     ptr = lambda t: t.data_ptr() if t.numel() else None
+    if deltas:
+        d_deltas = torch.empty((n_ev, 4), dtype=torch.int32, device=dev)
+        d_has = torch.empty(n_ev, dtype=torch.uint8, device=dev)
+        if accept.any():
+            _lib.check(L.mjx_mjai_fill_deltas_dev(n, text.data_ptr(), int(log_off[-1]), d_off.data_ptr(), int(augment),
+                                                  d_counts.data_ptr(), offs[0].data_ptr(), offs[2].data_ptr(), offs[3].data_ptr(),
+                                                  ptr(hdr), ptr(lines), n_ev, ptr(kyoku), n_k * KYOKU_WORDS, ptr(hora),
+                                                  n_h * HORA_WORDS, ptr(d_deltas), ptr(d_has), st), "mjx_mjai_fill_deltas_dev")
+        return DecodedLogs(accept, counts, ev_off, ev_cnt, ky_off, hora_off, offs, hdr, lines, kyoku, hora, d_deltas, d_has)
     if accept.any():
         _lib.check(L.mjx_mjai_fill_dev(n, text.data_ptr(), int(log_off[-1]), d_off.data_ptr(), int(augment), d_counts.data_ptr(),
                                        offs[0].data_ptr(), offs[2].data_ptr(), offs[3].data_ptr(), ptr(hdr), ptr(lines), n_ev,
