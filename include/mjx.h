@@ -135,6 +135,13 @@ int mjx_env_read_grp(mjx_env* env, void* stream, int32_t* feat_host, int32_t* n_
 int mjx_env_create_replay(mjx_env** out, int n_jobs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt, long long n_hdr,
                           const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words, const uint8_t* players,
                           int obs_version, int always_include_kan_select);
+/* The same with `hdr` and `kyoku` in DEVICE memory (e.g. the arrays of mjx_mjai_fill_dev, with host-encoded logs appended): they are
+ * copied device to device into the env's own buffers on `stream`, and the stream is synchronised before the call returns, so the
+ * caller may free them at once. ev_off, ev_cnt, ky_off and players stay host arrays; a job whose events lie outside [0, n_hdr) or
+ * whose first payload lies outside [0, n_kyoku_words / 19] fails the call with MJX_ERR_ARG. */
+int mjx_env_create_replay_dev(mjx_env** out, int n_jobs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt,
+                              long long n_hdr, const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words,
+                              const uint8_t* players, int obs_version, int always_include_kan_select, void* stream);
 int mjx_env_replay_step(mjx_env* env, void* stream);
 /* dataset/invisible.rs:35-66 (`trust_seed`): the logs were produced from known seeds (start_game.seed, what this arena and
  * libriichi's write) — host arrays (nonce, key) per job. Every kyoku's wall is then regenerated on device (board.rs:99-123), checked
@@ -246,6 +253,26 @@ enum mjx_stat_status { MJX_STAT_OK = 0, MJX_STAT_NOT_START_GAME = 1, MJX_STAT_NO
 int mjx_stat_logs_dev(int n_logs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt, long long n_hdr,
                       const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words, const int32_t* deltas,
                       const uint8_t* has_deltas, const uint8_t* seats, int64_t* out, int32_t* status, void* stream);
+
+/* ---- GRP targets of a log: dataset/grp.rs:90-164 Grp::load_events (csrc/mjx_grp.cuh) --------------------------------------------
+ * The per-log status: OK = the outputs are the log's Grp; otherwise the caller decides (mortal_b200/dataset.py runs the host
+ * Grp.load_events on such a log, which raises). NO_DELTAS: a hora or ryukyoku after the last start_kyoku has no usable deltas;
+ * NO_KYOKU: the log has no start_kyoku; CAPACITY: the log's events or start_kyoku payloads lie outside the arrays. */
+enum mjx_grp_status { MJX_GRP_OK = 0, MJX_GRP_NO_DELTAS = 1, MJX_GRP_NO_KYOKU = 2, MJX_GRP_CAPACITY = 3 };
+/* Grp.load_events of every log, over the arrays of mjx_mjai_fill_deltas_dev (device pointers): event words hdr [n_hdr] with
+ * ev_off / ev_cnt [n_logs]; start_kyoku payloads kyoku [n_kyoku_words] (19 words each, log i's first at ky_off[i]; the scores are
+ * words 0-1); deltas / has_deltas [n_hdr] as above. Outputs:
+ *   feat           int32 [n_kyoku_words / 19, 7]: the row of every start_kyoku at its payload index, {grand_kyoku (E1 = 0 .. S4 = 7,
+ *                  W and N rounds 7 + kyoku), honba, kyotaku, scores[4]} (the reference's f64 row is these with the scores divided
+ *                  by 10000); a log with a non-zero status may have some of its rows written;
+ *   rank_by_player uint8 [n_logs, 4] and final_scores int64 [n_logs, 4]: rankings.rs order (stable by seat), the sticks left on the
+ *                  table added to the leader; zero where the status is not OK;
+ *   status         int32 [n_logs] mjx_grp_status.
+ * One warp per log; enqueued on `stream` without a synchronise. Every read is bounded by n_hdr / n_kyoku_words. */
+int mjx_grp_logs_dev(int n_logs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt, long long n_hdr,
+                     const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words, const int32_t* deltas,
+                     const uint8_t* has_deltas, int32_t* feat, uint8_t* rank_by_player, int64_t* final_scores, int32_t* status,
+                     void* stream);
 
 /* ---- libriichi.state.PlayerState (state/player_state.rs:143-264, state/getter.rs:6-156, state/obs_repr.rs:776-791) ---------
  * A batch of n independent single-seat states: table records in single-seat mode (other seats' hidden tiles are `?` = 37), updated

@@ -71,6 +71,8 @@ SYMBOLS = {
     "mjx_nn_block_tail_bf16": (C.c_int, [C.c_void_p] * 11 + [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "mjx_env_create_replay": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p,
                                         C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_int]),
+    "mjx_env_create_replay_dev": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong,
+                                            C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "mjx_env_replay_trust_seeds": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "mjx_env_replay_step": (C.c_int, [C.c_void_p, C.c_void_p]),
     "mjx_env_row_label": (C.c_void_p, [C.c_void_p]),
@@ -108,6 +110,8 @@ SYMBOLS = {
                                            C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p]),
     "mjx_stat_logs_dev": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong,
                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mjx_grp_logs_dev": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong,
+                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 

@@ -12,6 +12,7 @@
 #include "mjx_validate.cuh"
 #include "mjx_mjai.cuh"
 #include "mjx_stat.cuh"
+#include "mjx_grp.cuh"
 #include "mjx_invisible.cuh"
 #include "mjx_state.cuh"
 #include "mjx_nn.cuh"
@@ -242,6 +243,24 @@ __global__ void __launch_bounds__(STAT_WARPS * 32) k_stat_logs(StatView V) {
     for (int k = lane; k < MJX_STAT_N; k += 32)
         V.out[(long long)i * MJX_STAT_N + k] = status ? 0 : c[0][k] + c[1][k] + c[2][k] + c[3][k];
     if (lane == 0) V.status[i] = status;
+}
+
+// GRP targets (csrc/mjx_grp.cuh): one warp = one log. The warp loads the event words 32 at a time (coalesced) and shuffles each to
+// every lane; lane 0 writes the feature rows, the ranking, the final scores and the status.
+__global__ void __launch_bounds__(GRP_WARPS * 32) k_grp_logs(GrpView V) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int i = blockIdx.x * GRP_WARPS + warp;
+    if (i >= V.n_logs) return;
+    u8 rank[4] = {0, 0, 0, 0};
+    i64 fin[4] = {0, 0, 0, 0};
+    const int status = grp_log(V, i, lane, rank, fin);
+    if (lane == 0) {
+        for (int k = 0; k < 4; k++) {
+            V.rank[4 * i + k] = status ? 0 : rank[k];
+            V.final[4 * i + k] = status ? 0 : fin[k];
+        }
+        V.status[i] = status;
+    }
 }
 
 __global__ void k_begin_step(EnvView V) {
@@ -1231,11 +1250,11 @@ int mjx_env_read_log(mjx_env* env, void* stream, uint64_t* words_host, int32_t* 
     return MJX_OK;
 }
 
-int mjx_env_create_replay(mjx_env** out, int n_jobs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt, long long n_hdr,
-                          const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words, const uint8_t* players,
-                          int obs_version, int always_include_kan_select) {
-    if (!out || n_jobs <= 0 || !hdr || !ev_off || !ev_cnt || !ky_off || !players || n_hdr <= 0)
-        return fail(MJX_ERR_ARG, "mjx_env_create_replay: bad arguments");
+// mjx_env_create_replay's body: `hdr` / `kyoku` are read with `kind` (host to device, or device to device) on `st`
+static int env_create_replay_impl(mjx_env** out, int n_jobs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt,
+                                  long long n_hdr, const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words,
+                                  const uint8_t* players, int obs_version, int always_include_kan_select, cudaMemcpyKind kind,
+                                  cudaStream_t st) {
     std::vector<uint64_t> zeros((size_t)n_jobs, 0);
     int rc = mjx_env_create(out, n_jobs, zeros.data(), zeros.data(), obs_version, 0, 0);
     if (rc) return rc;
@@ -1255,8 +1274,14 @@ int mjx_env_create_replay(mjx_env** out, int n_jobs, const uint64_t* hdr, const 
         CU(cudaMalloc(&R.ky_seen, sizeof(i32) * (size_t)n_jobs));
         CU(cudaMalloc(&R.row_label, sizeof(i64) * cap));
         CU(cudaMalloc(&R.row_meta, cap * 4));
-        CU(cudaMemcpy((void*)R.hdr, hdr, sizeof(u64) * (size_t)n_hdr, cudaMemcpyHostToDevice));
-        if (n_kyoku_words > 0) CU(cudaMemcpy((void*)R.kyoku, kyoku, sizeof(u64) * (size_t)n_kyoku_words, cudaMemcpyHostToDevice));
+        if (kind == cudaMemcpyHostToDevice) {
+            CU(cudaMemcpy((void*)R.hdr, hdr, sizeof(u64) * (size_t)n_hdr, cudaMemcpyHostToDevice));
+            if (n_kyoku_words > 0) CU(cudaMemcpy((void*)R.kyoku, kyoku, sizeof(u64) * (size_t)n_kyoku_words, cudaMemcpyHostToDevice));
+        } else {
+            CU(cudaMemcpyAsync((void*)R.hdr, hdr, sizeof(u64) * (size_t)n_hdr, kind, st));
+            if (n_kyoku_words > 0) CU(cudaMemcpyAsync((void*)R.kyoku, kyoku, sizeof(u64) * (size_t)n_kyoku_words, kind, st));
+            CU(cudaStreamSynchronize(st));
+        }
         CU(cudaMemcpy((void*)R.ev_off, ev_off, sizeof(i32) * (size_t)n_jobs, cudaMemcpyHostToDevice));
         CU(cudaMemcpy((void*)R.ev_cnt, ev_cnt, sizeof(i32) * (size_t)n_jobs, cudaMemcpyHostToDevice));
         CU(cudaMemcpy((void*)R.ky_off, ky_off, sizeof(i32) * (size_t)n_jobs, cudaMemcpyHostToDevice));
@@ -1269,6 +1294,29 @@ int mjx_env_create_replay(mjx_env** out, int n_jobs, const uint64_t* hdr, const 
     }();
     if (rc) return destroy_failed(out, env, rc);
     return MJX_OK;
+}
+
+int mjx_env_create_replay(mjx_env** out, int n_jobs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt, long long n_hdr,
+                          const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words, const uint8_t* players,
+                          int obs_version, int always_include_kan_select) {
+    if (!out || n_jobs <= 0 || !hdr || !ev_off || !ev_cnt || !ky_off || !players || n_hdr <= 0)
+        return fail(MJX_ERR_ARG, "mjx_env_create_replay: bad arguments");
+    return env_create_replay_impl(out, n_jobs, hdr, ev_off, ev_cnt, n_hdr, kyoku, ky_off, n_kyoku_words, players, obs_version,
+                                  always_include_kan_select, cudaMemcpyHostToDevice, nullptr);
+}
+
+int mjx_env_create_replay_dev(mjx_env** out, int n_jobs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt,
+                              long long n_hdr, const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words,
+                              const uint8_t* players, int obs_version, int always_include_kan_select, void* stream) {
+    if (!out || n_jobs <= 0 || !hdr || !ev_off || !ev_cnt || !ky_off || !players || n_hdr <= 0 || n_kyoku_words < 0 ||
+        n_kyoku_words % REPLAY_KYOKU_WORDS || (n_kyoku_words > 0 && !kyoku))
+        return fail(MJX_ERR_ARG, "mjx_env_create_replay_dev: bad arguments");
+    const long long n_payloads = n_kyoku_words / REPLAY_KYOKU_WORDS;
+    for (int j = 0; j < n_jobs; j++)
+        if (ev_off[j] < 0 || ev_cnt[j] < 0 || (long long)ev_off[j] + ev_cnt[j] > n_hdr || ky_off[j] < 0 || ky_off[j] > n_payloads)
+            return fail(MJX_ERR_ARG, "mjx_env_create_replay_dev: job " + std::to_string(j) + " lies outside the arrays");
+    return env_create_replay_impl(out, n_jobs, hdr, ev_off, ev_cnt, n_hdr, kyoku, ky_off, n_kyoku_words, players, obs_version,
+                                  always_include_kan_select, cudaMemcpyDeviceToDevice, (cudaStream_t)stream);
 }
 
 // ---- bin/validate_logs.rs
@@ -1395,6 +1443,24 @@ int mjx_stat_logs_dev(int n_logs, const uint64_t* hdr, const int32_t* ev_off, co
     V.n_kyoku = n_kyoku_words / REPLAY_KYOKU_WORDS; V.deltas = deltas; V.has_deltas = has_deltas; V.seats = seats; V.n_logs = n_logs;
     V.out = out; V.status = status;
     k_stat_logs<<<(n_logs + STAT_WARPS - 1) / STAT_WARPS, STAT_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+// ---- GRP targets (dataset/grp.rs Grp::load_events)
+int mjx_grp_logs_dev(int n_logs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt, long long n_hdr,
+                     const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words, const int32_t* deltas,
+                     const uint8_t* has_deltas, int32_t* feat, uint8_t* rank_by_player, int64_t* final_scores, int32_t* status,
+                     void* stream) {
+    if (n_logs <= 0 || !ev_off || !ev_cnt || !ky_off || !rank_by_player || !final_scores || !status || n_hdr < 0 ||
+        (n_hdr > 0 && (!hdr || !deltas || !has_deltas)) || n_kyoku_words < 0 || n_kyoku_words % REPLAY_KYOKU_WORDS ||
+        (n_kyoku_words > 0 && (!kyoku || !feat)))
+        return fail(MJX_ERR_ARG, "mjx_grp_logs_dev: bad arguments");
+    GrpView V;
+    V.hdr = hdr; V.ev_off = ev_off; V.ev_cnt = ev_cnt; V.n_hdr = n_hdr; V.kyoku = kyoku; V.ky_off = ky_off;
+    V.n_kyoku = n_kyoku_words / REPLAY_KYOKU_WORDS; V.deltas = deltas; V.has_deltas = has_deltas; V.n_logs = n_logs;
+    V.feat = feat; V.rank = rank_by_player; V.final = final_scores; V.status = status;
+    k_grp_logs<<<(n_logs + GRP_WARPS - 1) / GRP_WARPS, GRP_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
     CU(cudaGetLastError());
     return MJX_OK;
 }

@@ -298,7 +298,8 @@ class BatchEnv:
 
 class ReplayEnv(BatchEnv):
     """Replay mode (include/mjx.h mjx_env_create_replay): jobs = (game log, player) pairs advanced from logged decision to
-    logged decision; the encoder API of BatchEnv applies unchanged. `jobs` comes from mortal_b200.dataset_codec.build_jobs."""
+    logged decision; the encoder API of BatchEnv applies unchanged. `jobs` comes from mortal_b200.dataset_codec.build_jobs, or
+    has `hdr` and `kyoku` as int64 CUDA tensors of `device` (the decoder's arrays; mjx_env_create_replay_dev)."""
 
     def __init__(self, jobs, *, obs_version: int = 4, always_include_kan_select: bool = True, device: int = 0):
         import torch
@@ -310,15 +311,24 @@ class ReplayEnv(BatchEnv):
         torch.cuda.set_device(self.device)
         _lib.init(device)
         self.L = _lib.load()
-        j = {k: np.ascontiguousarray(v) for k, v in jobs.items()}
+        on_dev = isinstance(jobs["hdr"], torch.Tensor)  # hdr / kyoku already on the device (mjx_env_create_replay_dev)
+        j = {k: v if on_dev and k in ("hdr", "kyoku") else np.ascontiguousarray(v) for k, v in jobs.items()}
         self.n_tables = int(len(j["players"]))
         self.obs_version = obs_version
         self.obs_rows = self.L.mjx_obs_rows(obs_version)
         h = C.c_void_p()
-        _lib.check(self.L.mjx_env_create_replay(C.byref(h), self.n_tables, j["hdr"].ctypes.data, j["ev_off"].ctypes.data,
-                                                j["ev_cnt"].ctypes.data, len(j["hdr"]), j["kyoku"].ctypes.data,
-                                                j["ky_off"].ctypes.data, len(j["kyoku"]), j["players"].ctypes.data, obs_version,
-                                                int(always_include_kan_select)), "mjx_env_create_replay")
+        if on_dev:
+            hdr, ky = j["hdr"].contiguous(), j["kyoku"].contiguous()
+            _lib.check(self.L.mjx_env_create_replay_dev(C.byref(h), self.n_tables, hdr.data_ptr(), j["ev_off"].ctypes.data,
+                                                        j["ev_cnt"].ctypes.data, hdr.numel(), ky.data_ptr() if ky.numel() else None,
+                                                        j["ky_off"].ctypes.data, ky.numel(), j["players"].ctypes.data, obs_version,
+                                                        int(always_include_kan_select), torch.cuda.current_stream(self.device).cuda_stream),
+                       "mjx_env_create_replay_dev")
+        else:
+            _lib.check(self.L.mjx_env_create_replay(C.byref(h), self.n_tables, j["hdr"].ctypes.data, j["ev_off"].ctypes.data,
+                                                    j["ev_cnt"].ctypes.data, len(j["hdr"]), j["kyoku"].ctypes.data,
+                                                    j["ky_off"].ctypes.data, len(j["kyoku"]), j["players"].ctypes.data, obs_version,
+                                                    int(always_include_kan_select)), "mjx_env_create_replay")
         self._h = h
         self._bind_views()
         self.row_label = self._as_t(self.L.mjx_env_row_label(h), (self.row_cap,), "<i8")

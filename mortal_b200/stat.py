@@ -18,12 +18,14 @@ from __future__ import annotations
 import glob
 import gzip
 import json
-import locale
 import math
 import os
 import re
 import sys
 from concurrent.futures import ThreadPoolExecutor
+
+from . import _logio
+from ._logio import device_ready as _device_ready, log_device as _stat_device, read_bytes as _read_bytes  # noqa: F401
 
 COUNTERS = (
     "game round oya point rank_1 rank_2 rank_3 rank_4 tobi "
@@ -66,10 +68,9 @@ RATES = {
     "yakuman_rate": ("yakuman", "round"), "nagashi_mangan_rate": ("nagashi_mangan", "round"),
 }
 # from_dir's device path decodes and counts the files in chunks of consecutive files: at most CHUNK_LOGS files and, unless a
-# single file is larger, CHUNK_BYTES of decompressed text. The text of a chunk is held three times (the file contents, the pinned
-# staging buffer, the device copy), so this bounds memory whatever the corpus size.
-CHUNK_LOGS = 4096
-CHUNK_BYTES = 256 << 20
+# single file is larger, CHUNK_BYTES of decompressed text (_logio.py).
+CHUNK_LOGS = _logio.CHUNK_LOGS
+CHUNK_BYTES = _logio.CHUNK_BYTES
 
 
 def _fdiv(a: float, b: float) -> float:
@@ -307,32 +308,6 @@ def _read_counters():
     return tuple(re.findall(r"X\((\w+)\)", block))
 
 
-def _device_ready() -> bool:
-    """the device path needs the built library, a CUDA device, and a UTF-8 locale (the host path reads the files in the locale's
-    encoding; the decoder reads UTF-8)"""
-    from . import _lib
-
-    if not os.path.exists(_lib.lib_path()) or locale.getpreferredencoding(False).lower().replace("-", "") != "utf8":
-        return False
-    try:
-        import torch
-    except ImportError:
-        return False
-    return torch.cuda.is_available()
-
-
-def _read_bytes(path: str):
-    """a file's bytes, gunzipped for `.gz`; None when that fails (the host path then decides)"""
-    try:
-        if path.lower().endswith(".gz"):
-            with gzip.open(path, "rb") as f:
-                return f.read()
-        with open(path, "rb") as f:
-            return f.read()
-    except Exception:  # noqa: BLE001 — any failure: the host path raises its own exception for this file
-        return None
-
-
 def _seat_mask(blob: bytes, b: int, e: int, player_name: str):
     """the seats named player_name on a log's first event line (bytes [b, e)) as a bit mask, or None when the host must decide"""
     try:
@@ -347,31 +322,10 @@ def _seat_mask(blob: bytes, b: int, e: int, player_name: str):
     return sum(1 << i for i in seats)
 
 
-def _stat_device() -> int:
-    """the GPU from_dir runs on: the one libmjx is initialised on (the library serves one device per process, so a process whose
-    arena or engine lives on cuda:k counts there too), else torch's current device"""
-    from . import _lib
-
-    if _lib._INIT_DEVICE is not None:
-        return _lib._INIT_DEVICE
-    import torch
-
-    return torch.cuda.current_device()
-
-
 def _chunks(paths, pool, step: int):
     """(paths, contents) of consecutive files in order, read + gunzipped on `pool` `step` at a time, cut at CHUNK_LOGS files or
     CHUNK_BYTES of text (a chunk always takes at least one file)"""
-    cur, size, lo = [], 0, 0
-    for s in range(0, len(paths), step):
-        for b in pool.map(_read_bytes, paths[s:s + step]):
-            n = len(b) if b is not None else 0
-            if cur and (len(cur) >= CHUNK_LOGS or size + n > CHUNK_BYTES):
-                yield paths[lo:lo + len(cur)], cur
-                lo += len(cur); cur, size = [], 0
-            cur.append(b); size += n
-    if cur:
-        yield paths[lo:lo + len(cur)], cur
+    return _logio.chunks(paths, pool, step, _read_bytes, CHUNK_LOGS, CHUNK_BYTES)
 
 
 def _device_from_dir(paths, player_name: str, device: int | None = None) -> Stat:
