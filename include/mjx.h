@@ -128,8 +128,9 @@ int mjx_env_read_grp(mjx_env* env, void* stream, int32_t* feat_host, int32_t* n_
  * A job = one (game log, player). `hdr`: the games' events as 64-bit words (csrc/mjx_step.cuh `log_word`; start_game = 15,
  * end_game = 16), concatenated, job j owning ev_cnt[j] words from ev_off[j]; `kyoku`: 19 words per start_kyoku (2 of scores, 17 = the
  * 136-byte wall in board.rs:109-122 layout: the 52 dealt tiles, the rest `?` = 37 unless the hidden tiles are known),
- * job j's first payload at index ky_off[j]; `players`: the job's point of view. All host arrays. Full-information logs only.
- * mjx_env_replay_step advances every job to the next decision the log shows its player making and emits the row(s)
+ * job j's first payload at index ky_off[j]; `players`: the job's point of view. All host arrays. The record holds all four hands,
+ * so the logs must carry full information, unless mjx_env_replay_viewpoints (below) is called: then a log may hide the other
+ * seats' tiles (`?` = 37) as the mjai protocol shows a game to one seat. mjx_env_replay_step advances every job to the next decision the log shows its player making and emits the row(s)
  * (decision, then kan-select); observation / mask / row_table / row_seat are read exactly as after mjx_env_step, plus the
  * label and (at_kyoku, at_turn, shanten, apply_gamma) of each row. A job is finished when mjx_env_num_live stops counting it. */
 int mjx_env_create_replay(mjx_env** out, int n_jobs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt, long long n_hdr,
@@ -143,10 +144,21 @@ int mjx_env_create_replay_dev(mjx_env** out, int n_jobs, const uint64_t* hdr, co
                               long long n_hdr, const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words,
                               const uint8_t* players, int obs_version, int always_include_kan_select, void* stream);
 int mjx_env_replay_step(mjx_env* env, void* stream);
+/* dataset/gameplay.rs:240-335 with oracle = false (only the player's own PlayerState is updated): single-viewpoint logs. One launch,
+ * enqueued on `stream`, that scans every job's log for hidden seats: a seat is hidden when one of its 13 haipai tiles in a
+ * start_kyoku payload, or the pai of one of its tsumo events, is `?` (37). A job whose log hides no seat is left exactly as it
+ * was (bit-identical replay). Otherwise the job is replayed from its player's own PlayerState (TableState.viewer1), and when the
+ * hidden seats include the player's own, the job fails at its first mjx_env_replay_step with the per-job error code
+ * MJX_REPLAY_ERR_HIDDEN_OWN_TILE (state/update.rs:695-699: "attempt to witness an unknown tile"). A job with more start_kyoku
+ * events than payloads left after ky_off[j] is not marked. Call after mjx_env_create_replay[_dev] and before the first
+ * mjx_env_replay_step; MJX_ERR_ARG on an env that is not a replay env or after mjx_env_replay_trust_seeds (trusted walls are for
+ * the invisible observation, whose logs stay full-information), MJX_ERR_STATE after the first step. */
+#define MJX_REPLAY_ERR_HIDDEN_OWN_TILE 13
+int mjx_env_replay_viewpoints(mjx_env* env, void* stream);
 /* dataset/invisible.rs:35-66 (`trust_seed`): the logs were produced from known seeds (start_game.seed, what this arena and
  * libriichi's write) — host arrays (nonce, key) per job. Every kyoku's wall is then regenerated on device (board.rs:99-123), checked
  * against the logged haipai / dora marker (a mismatch fails the job), and mjx_env_encode_invisible can show the hidden tiles.
- * Call before the first mjx_env_replay_step. */
+ * Call before the first mjx_env_replay_step, and not after mjx_env_replay_viewpoints (MJX_ERR_ARG). */
 int mjx_env_replay_trust_seeds(mjx_env* env, const uint64_t* nonces_host, const uint64_t* keys_host, int shuffle_kind);
 int64_t* mjx_env_row_label(mjx_env* env); /* int64 [row_cap] device */
 uint8_t* mjx_env_row_meta(mjx_env* env);  /* uint8 [row_cap, 4] device: at_kyoku, at_turn, shanten (int8), apply_gamma */

@@ -75,6 +75,7 @@ SYMBOLS = {
                                             C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "mjx_env_replay_trust_seeds": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "mjx_env_replay_step": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "mjx_env_replay_viewpoints": (C.c_int, [C.c_void_p, C.c_void_p]),
     "mjx_env_row_label": (C.c_void_p, [C.c_void_p]),
     "mjx_env_row_meta": (C.c_void_p, [C.c_void_p]),
     "mjx_env_set_encode_timing": (C.c_int, [C.c_void_p, C.c_int]),

@@ -85,6 +85,19 @@ __global__ void __launch_bounds__(STEP_WARPS * 32) k_replay_step(EnvView V, Repl
     if (lane == 0 && live) atomicAdd(&V.counters[0], 1ull);
 }
 
+// Single-viewpoint logs (csrc/mjx_replay.cuh replay_hidden_seats): one warp = one replay job, run once before the first replay
+// step. The warp scans the job's event words and haipai for `?` seats; lane 0 marks the record (viewer1, ERR_HIDDEN_OWN_TILE).
+constexpr int VIEW_WARPS = 4;
+static_assert(ERR_HIDDEN_OWN_TILE == MJX_REPLAY_ERR_HIDDEN_OWN_TILE, "include/mjx.h documents the code");
+__global__ void __launch_bounds__(VIEW_WARPS * 32) k_replay_viewpoints(TableState* tabs, ReplayView R, int n_jobs, long long n_hdr,
+                                                                       long long n_kyoku) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int job = blockIdx.x * VIEW_WARPS + warp;
+    if (job >= n_jobs) return;
+    const int mask = replay_hidden_seats(R, job, n_hdr, n_kyoku, lane);
+    if (lane == 0) replay_mark_viewpoint(tabs + job, R.player[job], mask);
+}
+
 // Log validation (csrc/mjx_validate.cuh): one warp = one whole log. The record is initialised in shared memory and never
 // written back; the only store is the 16-byte verdict.
 __global__ void __launch_bounds__(STEP_WARPS * 32) k_validate_logs(ValidateView V, Tables T, long long n_hdr) {
@@ -768,6 +781,8 @@ struct mjx_env {
     bool time_encode = false;
     ReplayView R{};  // replay mode (mjx_env_create_replay): device arrays of the jobs
     bool replay = false;
+    long long r_n_hdr = 0, r_n_kyoku = 0;  // capacities of R.hdr (words) and R.kyoku (payloads)
+    bool viewpoints = false;              // mjx_env_replay_viewpoints was called
     int* d_enc_work = nullptr;  // k_encode_features' dynamic work counter
     EncStoreArgs enc_args{};
     cudaStream_t copy_stream = nullptr;  // mjx_env_encode_obs_host: D2H overlapped with the SP kernels
@@ -1290,6 +1305,8 @@ static int env_create_replay_impl(mjx_env** out, int n_jobs, const uint64_t* hdr
         CU(cudaMemset(R.ky_idx, 0, sizeof(i32) * (size_t)n_jobs));
         CU(cudaMemset(R.ky_seen, 0, sizeof(i32) * (size_t)n_jobs));
         R.always_include_kan_select = always_include_kan_select ? 1 : 0;
+        env->r_n_hdr = n_hdr;
+        env->r_n_kyoku = n_kyoku_words > 0 ? n_kyoku_words / REPLAY_KYOKU_WORDS : 0;
         return MJX_OK;
     }();
     if (rc) return destroy_failed(out, env, rc);
@@ -1556,6 +1573,7 @@ int mjx_env_replay_trust_seeds(mjx_env* env, const uint64_t* nonces_host, const 
     if (!env || !env->replay || !nonces_host || !keys_host) return fail(MJX_ERR_ARG, "mjx_env_replay_trust_seeds: bad arguments");
     if (!env->first) return fail(MJX_ERR_STATE, "mjx_env_replay_trust_seeds: must be called before the first mjx_env_replay_step");
     if (shuffle_kind != 0 && shuffle_kind != 1) return fail(MJX_ERR_ARG, "mjx_env_replay_trust_seeds: shuffle_kind must be 0 or 1");
+    if (env->viewpoints) return fail(MJX_ERR_ARG, "mjx_env_replay_trust_seeds: not with mjx_env_replay_viewpoints (full-information logs only)");
     const size_t n = (size_t)env->n_tables;
     CU(cudaMemcpy(env->d_nonces, nonces_host, sizeof(u64) * n, cudaMemcpyHostToDevice));
     CU(cudaMemcpy(env->d_keys, keys_host, sizeof(u64) * n, cudaMemcpyHostToDevice));
@@ -1563,6 +1581,18 @@ int mjx_env_replay_trust_seeds(mjx_env* env, const uint64_t* nonces_host, const 
     CU(cudaGetLastError());
     CU(cudaDeviceSynchronize());
     env->R.trust_seed = 1;
+    return MJX_OK;
+}
+
+int mjx_env_replay_viewpoints(mjx_env* env, void* stream) {
+    if (!env || !env->replay) return fail(MJX_ERR_ARG, "mjx_env_replay_viewpoints: not a replay env");
+    if (env->R.trust_seed) return fail(MJX_ERR_ARG, "mjx_env_replay_viewpoints: not with mjx_env_replay_trust_seeds (full-information logs only)");
+    if (!env->first) return fail(MJX_ERR_STATE, "mjx_env_replay_viewpoints: must be called before the first mjx_env_replay_step");
+    k_replay_viewpoints<<<(env->n_tables + VIEW_WARPS - 1) / VIEW_WARPS, VIEW_WARPS * 32, 0, (cudaStream_t)stream>>>(
+        env->V.tables, env->R, env->n_tables, env->r_n_hdr, env->r_n_kyoku);
+    CU(cudaGetLastError());
+    env->launches += 1;
+    env->viewpoints = true;
     return MJX_OK;
 }
 

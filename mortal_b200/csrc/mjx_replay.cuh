@@ -2,8 +2,9 @@
 //
 // A "job" = one (game log, player) pair. The log is a sequence of the same 64-bit event words k_step records
 // (csrc/mjx_step.cuh log_word; start_kyoku payloads in a side array). One warp replays one job through the very event
-// handlers self-play uses (the record holds all four seats; full-information logs as Mortal's arena or tenhou
-// conversions produce them), stops whenever the log shows the player making a decision, emits the decision row(s)
+// handlers self-play uses (the record holds all four seats for full-information logs as Mortal's arena or tenhou
+// conversions produce them; after k_replay_viewpoints, a log that hides the other seats' tiles, as the mjai protocol shows a
+// game to one seat, is replayed from the player's own PlayerState), stops whenever the log shows the player making a decision, emits the decision row(s)
 // with the label the following events imply (gameplay.rs:303-423) and lets the ordinary encoder kernels produce the
 // observation before the next call continues.
 #pragma once
@@ -121,6 +122,61 @@ MJX_DN void replay_apply(Ctx& c, const ReplayView& R, int job, u64 w) {
         MJX_L0(R.ky_seen[job] = seen + 1);
     }
     apply_event(c, w, pay, R.trust_seed != 0);
+}
+
+// Single-viewpoint logs (k_replay_viewpoints, mjx_env_replay_viewpoints): the seats job `job`'s log hides, bit s when one of
+// seat s's 13 haipai bytes in a start_kyoku payload, or the pai of one of its tsumo words, is `?` (what an mjai client is shown
+// of the other seats). -1 = leave the job as it is: its events lie outside [0, n_hdr), or it has more start_kyoku words than
+// payloads are left in [ky_off, n_kyoku) (n_kyoku counts payloads). Device: the warp loads the words 32 at a time (coalesced),
+// one per lane; a ballot prefix gives each start_kyoku lane its payload, whose haipai words (2..8) it reads. The result is
+// warp-uniform. -DMJX_HOST_EMUL walks the words on one lane.
+MJX_D unsigned hidden_seats_of_word(const ReplayView& R, u64 w, long long k, long long n_kyoku, bool& over) {
+    if (lw_type(w) == LOG_TSUMO) return lw_pai(w) == T_UNK ? 1u << lw_actor(w) : 0u;
+    if (lw_type(w) != LOG_START_KYOKU) return 0u;
+    if (k < 0 || k >= n_kyoku) { over = true; return 0u; }
+    const u64* hp = R.kyoku + k * REPLAY_KYOKU_WORDS + 2;
+    unsigned m = 0;
+    for (int i = 0; i < 52; i++)
+        if (((hp[i / 8] >> (8 * (i % 8))) & 0xFF) == T_UNK) m |= 1u << (i / 13);
+    return m;
+}
+
+MJX_DM int replay_hidden_seats(const ReplayView& R, int job, long long n_hdr, long long n_kyoku, int lane) {
+    const long long off = R.ev_off[job], cnt = R.ev_cnt[job];
+    if (off < 0 || cnt < 0 || off + cnt > n_hdr) return -1;
+    long long ky = R.ky_off[job];  // the next start_kyoku's payload
+    unsigned mask = 0;
+    bool over = false;
+    for (long long base = 0; base < cnt; base += 32) {
+        const int n = cnt - base < 32 ? (int)(cnt - base) : 32;
+#ifdef MJX_HOST_EMUL
+        (void)lane;
+        for (int j = 0; j < n; j++) {
+            const u64 w = R.hdr[off + base + j];
+            mask |= hidden_seats_of_word(R, w, ky, n_kyoku, over);
+            ky += lw_type(w) == LOG_START_KYOKU;
+        }
+#else
+        const u64 w = lane < n ? R.hdr[off + base + lane] : 0;  // type 0: no event
+        const unsigned sk = __ballot_sync(~0u, lw_type(w) == LOG_START_KYOKU);
+        mask |= hidden_seats_of_word(R, w, ky + __popc(sk & ((1u << lane) - 1)), n_kyoku, over);
+        ky += __popc(sk);
+#endif
+    }
+#ifndef MJX_HOST_EMUL
+    mask = __reduce_or_sync(~0u, mask);
+    over = __any_sync(~0u, over);
+#endif
+    return over ? -1 : (int)mask;
+}
+
+// The job's record after the scan: a log that hides a seat is replayed from the player's own PlayerState (viewer1 = player + 1;
+// dataset/gameplay.rs:240-335 with oracle = false runs only that state), and fails at once with ERR_HIDDEN_OWN_TILE when it hides
+// the player's own tiles. A full-information log (mask 0) and an unmarked job (-1) are left untouched.
+MJX_D void replay_mark_viewpoint(TableState* S, int player, int mask) {
+    if (mask <= 0 || player > 3) return;
+    S->viewer1 = (u8)(player + 1);
+    if (((mask >> player) & 1) && S->err == 0) S->err = ERR_HIDDEN_OWN_TILE;
 }
 
 // Advance one job to its next logged decision. Returns true while the job still has events to process.

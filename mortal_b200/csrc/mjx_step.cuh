@@ -28,6 +28,7 @@ enum : i32 {
     ERR_NONE = 0, ERR_ILLEGAL_ACTION = 1, ERR_KAWA_OVERFLOW = 2, ERR_WALL_EXHAUSTED = 3, ERR_FIFTH_KAN = 4,
     ERR_INTERNAL = 5, ERR_FOUR_WIND_STATE = 6, ERR_NO_KAWA_TILE = 7, ERR_ROW_OVERFLOW = 8, ERR_BAD_POINT = 9,
     ERR_KAN_CHOICE = 10, ERR_GUARD_NEEDS_Q = 11, ERR_SEED_MISMATCH = 12,
+    ERR_HIDDEN_OWN_TILE = 13,  // a replayed log hides the player's own tiles (state/update.rs:695-699 "witness an unknown tile")
 };
 
 struct WarpScratch {

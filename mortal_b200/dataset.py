@@ -6,7 +6,13 @@ always_include_kan_select, augmented)`, `.load_gz_log_files(filenames) -> list[l
 take_shantens / take_player_id`. The logs are replayed on device (csrc/mjx_replay.cuh) and the observations come from the
 same encoder kernels self-play uses. Differences, stated rather than hidden: `take_obs()` / `take_masks()` return ONE tensor
 per Gameplay ([n_moves, C, 34] float32 / [n_moves, 46] bool, CUDA by default, `host=True` for numpy) instead of a list of
-per-move arrays (`take_invisible_obs()` likewise: [n_moves, 217 | 211, 34]); logs must carry full information (no "?" tiles).
+per-move arrays (`take_invisible_obs()` likewise: [n_moves, 217 | 211, 34]).
+
+With `oracle=False` a log may hide the other seats' tiles, as the mjai protocol shows a game to one seat (their haipai "?" in
+start_kyoku, their draws "pai": "?"): as in the reference, only the selected player's own PlayerState is updated, so such a log
+loads for the seat that recorded it (select it with `player_names`) to exactly the Gameplays that seat has in the full log. A
+player whose own tiles are hidden fails the call with a RuntimeError (mjx error code 13), so the default selection of all four
+seats fails on such a log, as it does in the reference. With `oracle=True` every log must carry full information.
 With `oracle=True` the hidden tiles come from the game seed when `trust_seed=True` (walls regenerated on device and checked
 against the logged deal) and otherwise from the log plus a random fill of the unseen tiles, as dataset/invisible.rs does.
 `Grp` (dataset/grp.rs:19-164) is restated in Python (Grp.load_events) and, for whole batches of logs, on the device (k_grp_logs,
@@ -29,6 +35,8 @@ import numpy as np
 
 from . import _logio, dataset_codec
 from .env import ReplayEnv
+
+_ERR_HIDDEN_OWN_TILE = 13  # include/mjx.h MJX_REPLAY_ERR_HIDDEN_OWN_TILE
 
 
 class Grp:
@@ -309,6 +317,8 @@ class GameplayLoader:
                         raise ValueError("trust_seed=True needs start_game.seed in every log")
                     seeds.append((int(sd[0]), int(sd[1])))
                 env.trust_seeds([seeds[g][0] for g in jobs["job_game"]], [seeds[g][1] for g in jobs["job_game"]], self.shuffle_kind)
+            elif not self.oracle:  # gameplay.rs:240-335: only the player's own PlayerState is updated, so other seats may be `?`
+                env.viewpoints()
             while True:
                 env.replay_step()
                 nr = env.num_rows()
@@ -330,8 +340,12 @@ class GameplayLoader:
                                "would be zero; load fewer logs per call")
         if (res["err"] != 0).any():
             bad = int(np.nonzero(res["err"])[0][0])
+            code = int(res["err"][bad])
+            why = ("the player's own tiles are hidden in this log (attempt to witness an unknown tile); a log recorded from one "
+                   "seat loads for that seat only, selected with player_names" if code == _ERR_HIDDEN_OWN_TILE
+                   else "the log is inconsistent or not full-information")
             raise RuntimeError(f"replay job {bad} (log {int(jobs['job_game'][bad])}, player {int(jobs['players'][bad])}) failed "
-                               f"with mjx error code {int(res['err'][bad])}: the log is inconsistent or not full-information")
+                               f"with mjx error code {code}: {why}")
         if chunks:
             job = torch.cat([c[0] for c in chunks]); obs = torch.cat([c[1] for c in chunks]); masks = torch.cat([c[2] for c in chunks])
             label = torch.cat([c[3] for c in chunks]); meta = torch.cat([c[4] for c in chunks])

@@ -341,5 +341,11 @@ class ReplayEnv(BatchEnv):
         assert n_.shape == k_.shape == (self.n_tables,)
         _lib.check(self.L.mjx_env_replay_trust_seeds(self._h, n_.ctypes.data, k_.ctypes.data, shuffle_kind), "mjx_env_replay_trust_seeds")
 
+    def viewpoints(self) -> None:
+        """Single-viewpoint logs (mjx_env_replay_viewpoints): a job whose log hides other seats' tiles (`?` haipai or tsumo) replays
+        from its player's own PlayerState, and fails with error code 13 when it hides the player's own tiles. Full-information logs
+        replay exactly as without the call. Call before the first replay_step; not together with trust_seeds."""
+        _lib.check(self.L.mjx_env_replay_viewpoints(self._h, self._stream()), "mjx_env_replay_viewpoints")
+
     def replay_step(self) -> None:
         _lib.check(self.L.mjx_env_replay_step(self._h, self._stream()), "mjx_env_replay_step")
