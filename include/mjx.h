@@ -115,6 +115,48 @@ int mjx_env_enable_log(mjx_env* env, int words_per_table);
 int mjx_env_read_log(mjx_env* env, void* stream, uint64_t* words_host, int32_t* len_host);
 int32_t* mjx_env_log_len_dev(mjx_env* env); /* int32 [n_tables] device view of the per-table word counts (null before enable_log):
                                               read after every step it tells which events that step wrote (per-decision meta) */
+uint64_t* mjx_env_log_words_dev(mjx_env* env); /* uint64 [n_tables, words_per_table] device view of the words (null before
+                                                  enable_log); words past a table's count are undefined */
+
+/* ---- mjai log text from the event words: mortal_b200/mjai_log.py decode_events + attach_meta + dump_json_log (csrc/mjx_mjai_write.cuh)
+ * Every game's event lines, byte for byte what the host writer produces between its start_game and end_game lines (those carry the
+ * names and the seed and are rendered by the caller). Device pointers, enqueued on `stream` without a synchronise; one warp per game.
+ *   words   uint64 [n_games, log_cap] and lens int32 [n_games] (mjx_env_log_words_dev / mjx_env_log_len_dev);
+ *   bounds  int32 [n_steps, n_games]: game g's word count right after environment step c (null or n_rec == 0: no meta);
+ *   records one per decision row, sorted by key = ((game * key_steps + step) * 4 + seat) * 2 + kan_select (key_steps > every step):
+ *           rec_info int32 [n_rec, 4] = {action, MJX_MW_REC_* flags, shanten, row order}, rec_mask uint64 [n_rec] (46 legal bits),
+ *           rec_q float32 [n_rec, 46], rec_i64 int64 [n_rec, 2] = {batch_size, eval_time_ns}.
+ * An agent event at word offset `off` takes the record of (game, step = bisect_right(bounds[:, g], off) - 1, actor, 0) when that
+ * record's action produces the event type (ryukyoku: the seat whose action is 44); action 42 nests the (…, 1) record as kan_select.
+ *   mjx_mjai_render_count_dev -> bytes int32 [n_games] (the text length), status int32 [n_games] (mjx_mw_status: non-zero = the host
+ *                                writer raises on this game; its bytes are then 0);
+ *   mjx_mjai_render_fill_dev  the text of games [g0, g1) with status OK: game g at out + off[g] - off[g0] (off int64 [n_games + 1],
+ *                                the exclusive sum of bytes); nothing is written at or past out_cap.
+ * Reads never pass a game's log_cap words. */
+/* Per-decision meta records for the renderer, appended on the device on `stream` (no synchronise): for the i-th of the n rows of an
+ * agent call (row = idx[i], or i when idx is null), record base + i gets the row's table (row_table), `cycle`, seat | kan_select << 2
+ * (row_seat), out_info {actions[row], MJX_MW_REC_* flags (greedy[i], or greedy when null; shanten / furiten when obs is given),
+ * shanten = the first maximum of obs rows 862-868 at column 0, row}, the 46 legal bits of masks[row], the call's Q-values q[i]
+ * (float32 [n, 46], call order) and call_ids[i] (or `call`). obs: float32 [row_cap, obs_rows, 34] v4 observation or null. Fails
+ * with MJX_ERR_ARG, writing nothing, unless base + n <= cap; a row index outside row_cap gives a record no event matches. */
+int mjx_meta_record_dev(long long n, const int64_t* idx, const float* q, const uint8_t* greedy, const int32_t* call_ids, int call,
+                        int cycle, const int32_t* row_table, const uint8_t* row_seat, const int64_t* actions, const uint8_t* masks,
+                        const float* obs, int obs_rows, int row_cap, int32_t* out_table, int32_t* out_cycle, uint8_t* out_seat,
+                        int32_t* out_info, uint64_t* out_mask, float* out_q, int32_t* out_call, long long base, long long cap,
+                        void* stream);
+enum mjx_mw_status { MJX_MW_OK = 0, MJX_MW_CORRUPT = 1, MJX_MW_TRUNCATED = 2, MJX_MW_CAPACITY = 3 };
+enum mjx_mw_event { MJX_MW_T_START_KYOKU = 1, MJX_MW_T_TSUMO, MJX_MW_T_DAHAI, MJX_MW_T_CHI, MJX_MW_T_PON, MJX_MW_T_DAIMINKAN,
+                    MJX_MW_T_KAKAN, MJX_MW_T_ANKAN, MJX_MW_T_DORA, MJX_MW_T_REACH, MJX_MW_T_REACH_ACCEPTED, MJX_MW_T_HORA,
+                    MJX_MW_T_RYUKYOKU, MJX_MW_T_END_KYOKU };
+enum mjx_mw_rec_flag { MJX_MW_REC_GREEDY = 1, MJX_MW_REC_HAS_SHANTEN = 2, MJX_MW_REC_HAS_FURITEN = 4, MJX_MW_REC_FURITEN = 8 };
+int mjx_mjai_render_count_dev(int n_games, const uint64_t* words, const int32_t* lens, int log_cap, const int32_t* bounds,
+                              int n_steps, int key_steps, const int64_t* rec_key, const int32_t* rec_info, const uint64_t* rec_mask,
+                              const float* rec_q, const int64_t* rec_i64, long long n_rec, int32_t* bytes, int32_t* status,
+                              void* stream);
+int mjx_mjai_render_fill_dev(int n_games, const uint64_t* words, const int32_t* lens, int log_cap, const int32_t* bounds,
+                             int n_steps, int key_steps, const int64_t* rec_key, const int32_t* rec_info, const uint64_t* rec_mask,
+                             const float* rec_q, const int64_t* rec_i64, long long n_rec, const int32_t* status, const int64_t* off,
+                             int g0, int g1, char* out, long long out_cap, void* stream);
 
 /* dataset/grp.rs:90-164 without the logs: the GRP feature row of every kyoku — {grand_kyoku (E1 = 0 .. S4 = 7, W = 8+), honba,
  * kyotaku, scores[4]} as int32 (the reference's f64 row is these with the scores divided by 10000) — is written by the step

@@ -64,6 +64,15 @@ SYMBOLS = {
     "mjx_env_enable_log": (C.c_int, [C.c_void_p, C.c_int]),
     "mjx_env_log_len_dev": (C.c_void_p, [C.c_void_p]),
     "mjx_env_read_log": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mjx_env_log_words_dev": (C.c_void_p, [C.c_void_p]),
+    "mjx_meta_record_dev": (C.c_int, [C.c_longlong] + [C.c_void_p] * 4 + [C.c_int, C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_int]
+                            + [C.c_void_p] * 7 + [C.c_longlong, C.c_longlong, C.c_void_p]),
+    "mjx_mjai_render_count_dev": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p,
+                                            C.c_void_p]),
+    "mjx_mjai_render_fill_dev": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p,
+                                           C.c_int, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p]),
     "mjx_nn_affine_mish_bf16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_void_p]),
     "mjx_nn_pool_bf16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "mjx_nn_gate_residual_bf16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),

@@ -11,6 +11,7 @@
 #include "mjx_replay.cuh"
 #include "mjx_validate.cuh"
 #include "mjx_mjai.cuh"
+#include "mjx_mjai_write.cuh"
 #include "mjx_stat.cuh"
 #include "mjx_grp.cuh"
 #include "mjx_invisible.cuh"
@@ -1010,6 +1011,100 @@ static int destroy_failed(mjx_env** out, mjx_env* env, int rc) {
     return rc;
 }
 
+// ---- per-decision meta records: one warp per decision row of an agent call (lane a < 46 and 32 + a hold action a)
+__global__ void __launch_bounds__(MW_WARPS * 32) k_meta_record(MrView V) {
+    const int lane = threadIdx.x & 31;
+    const long long i = (long long)blockIdx.x * MW_WARPS + (threadIdx.x >> 5);
+    if (i >= V.n) return;
+    int r;
+    long long o;
+    if (!mr_head(V, i, &r, &o)) return;
+    bool m0 = false, m1 = false;
+    if (r >= 0) {
+        const u8* mk = V.masks + (long long)r * 46;
+        m0 = mk[lane] != 0;
+        m1 = lane < 14 && mk[32 + lane] != 0;
+        V.out_q[o * 46 + lane] = V.q[i * 46 + lane];
+        if (lane < 14) V.out_q[o * 46 + 32 + lane] = V.q[i * 46 + 32 + lane];
+    } else {
+        V.out_q[o * 46 + lane] = 0.f;
+        if (lane < 14) V.out_q[o * 46 + 32 + lane] = 0.f;
+    }
+    const u64 mask = (u64)__ballot_sync(~0u, m0) | ((u64)__ballot_sync(~0u, m1) << 32);
+    if (lane == 0) mr_fields(V, i, r, o, mask);
+}
+
+// ---- event words -> mjai log text (mjai_log.py decode_events + attach_meta + dump_json_log)
+// One game per warp. Lane 0 queues the next 32 event starts, each lane sizes one event, a warp prefix sum places them; FILL
+// writes them there. The walk, the statuses and the byte counts are warp-uniform.
+template <bool FILL>
+__global__ void __launch_bounds__(MW_WARPS * 32) k_mjai_render(MwView V) {
+    __shared__ int s_start[MW_WARPS][32];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const int g = (FILL ? V.g0 : 0) + blockIdx.x * MW_WARPS + wid;
+    if (g >= (FILL ? V.g1 : V.n_games)) return;
+    if (FILL && V.status[g] != MJX_MW_OK) return;
+    const u64* w;
+    int n;
+    int st = mw_game_words(V, g, &w, &n);
+    const long long base = FILL ? V.off[g] - V.off[V.g0] : 0;
+    long long total = 0;
+    for (int pos = 0; st == MJX_MW_OK && pos < n;) {
+        int cnt = 0, nx = pos, wst = MJX_MW_OK;
+        if (lane == 0) {
+            while (cnt < 32 && nx < n) {
+                const int t = mw_next(w, n, nx);
+                if (t < 0) { wst = -t; break; }
+                s_start[wid][cnt++] = nx;
+                nx = t;
+            }
+        }
+        __syncwarp();
+        cnt = __shfl_sync(~0u, cnt, 0);
+        nx = __shfl_sync(~0u, nx, 0);
+        wst = __shfl_sync(~0u, wst, 0);
+        int size = 0, est = MJX_MW_OK;
+        if (lane < cnt) {
+            MwOut o{nullptr, 0, 0};
+            est = mw_event(o, V, g, w, s_start[wid][lane]);
+            size = (int)o.n;
+        }
+        const unsigned bad = __ballot_sync(~0u, est != MJX_MW_OK);
+        if (bad) est = __shfl_sync(~0u, est, __ffs(bad) - 1);
+        int incl = size;
+        for (int d = 1; d < 32; d <<= 1) {
+            const int v = __shfl_up_sync(~0u, incl, d);
+            if (lane >= d) incl += v;
+        }
+        if (FILL && !bad && lane < cnt) {
+            const long long at = base + total + incl - size;
+            MwOut o{V.out + at, 0, V.out_cap - at};
+            mw_event(o, V, g, w, s_start[wid][lane]);
+        }
+        total += __shfl_sync(~0u, incl, 31);
+        __syncwarp();  // s_start is refilled by lane 0
+        st = bad ? est : wst;
+        pos = nx;
+    }
+    if (!FILL && lane == 0) {
+        V.status[g] = st;
+        V.bytes[g] = st == MJX_MW_OK ? (i32)total : 0;
+    }
+}
+
+static bool mw_view(MwView& V, int n_games, const uint64_t* words, const int32_t* lens, int log_cap, const int32_t* bounds, int n_steps,
+                    int key_steps, const int64_t* rec_key, const int32_t* rec_info, const uint64_t* rec_mask, const float* rec_q,
+                    const int64_t* rec_i64, long long n_rec) {
+    if (n_games <= 0 || !words || !lens || log_cap <= 0 || n_rec < 0) return false;
+    const bool meta = bounds && n_rec > 0;
+    if (meta && (n_steps <= 0 || key_steps < n_steps || !rec_key || !rec_info || !rec_mask || !rec_q || !rec_i64)) return false;
+    V = MwView{};
+    V.words = words; V.lens = lens; V.log_cap = log_cap; V.n_games = n_games;
+    V.bounds = meta ? bounds : nullptr; V.n_steps = meta ? n_steps : 0; V.key_steps = key_steps;
+    V.rec_key = rec_key; V.rec_info = rec_info; V.rec_mask = rec_mask; V.rec_q = rec_q; V.rec_i64 = rec_i64; V.n_rec = meta ? n_rec : 0;
+    return true;
+}
+
 extern "C" {
 
 int mjx_env_create(mjx_env** out, int n_tables, const uint64_t* nonces, const uint64_t* keys, int obs_version,
@@ -1254,6 +1349,7 @@ int mjx_env_read_grp(mjx_env* env, void* stream, int32_t* feat_host, int32_t* n_
 }
 
 int32_t* mjx_env_log_len_dev(mjx_env* env) { return env ? env->V.log_len : nullptr; }
+uint64_t* mjx_env_log_words_dev(mjx_env* env) { return env ? env->V.log : nullptr; }
 
 int mjx_env_read_log(mjx_env* env, void* stream, uint64_t* words_host, int32_t* len_host) {
     if (!env || !words_host || !len_host) return fail(MJX_ERR_ARG, "mjx_env_read_log: bad arguments");
@@ -1443,6 +1539,52 @@ int mjx_mjai_fill_deltas_dev(int n_logs, const uint8_t* text, long long n_bytes,
     V.n_hdr = n_hdr; V.n_kyoku = n_kyoku_words / REPLAY_KYOKU_WORDS; V.n_hora = n_hora_words / MJX_HORA_WORDS;
     k_mjai_decode<true, true><<<(n_logs + MJAI_WARPS - 1) / MJAI_WARPS, MJAI_WARPS * 32, 0, (cudaStream_t)stream>>>(
         V, MjaiDeltas{deltas, has_deltas});
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+// ---- per-decision meta records (k_meta_record)
+int mjx_meta_record_dev(long long n, const int64_t* idx, const float* q, const uint8_t* greedy, const int32_t* call_ids, int call,
+                        int cycle, const int32_t* row_table, const uint8_t* row_seat, const int64_t* actions, const uint8_t* masks,
+                        const float* obs, int obs_rows, int row_cap, int32_t* out_table, int32_t* out_cycle, uint8_t* out_seat,
+                        int32_t* out_info, uint64_t* out_mask, float* out_q, int32_t* out_call, long long base, long long cap,
+                        void* stream) {
+    if (n < 0 || (n > 0 && !q) || !row_table || !row_seat || !actions || !masks || (obs && obs_rows < 869) || row_cap <= 0 ||
+        !out_table || !out_cycle || !out_seat || !out_info || !out_mask || !out_q || !out_call || base < 0 || base + n > cap)
+        return fail(MJX_ERR_ARG, "mjx_meta_record_dev: bad arguments");
+    if (n == 0) return MJX_OK;
+    MrView V{n, idx, q, greedy, call_ids, call, cycle, row_table, row_seat, actions, masks, obs, obs_rows, row_cap,
+             out_table, out_cycle, out_seat, out_info, out_mask, out_q, out_call, base, cap};
+    k_meta_record<<<(unsigned)((n + MW_WARPS - 1) / MW_WARPS), MW_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+// ---- event words -> mjai log text (k_mjai_render)
+int mjx_mjai_render_count_dev(int n_games, const uint64_t* words, const int32_t* lens, int log_cap, const int32_t* bounds,
+                              int n_steps, int key_steps, const int64_t* rec_key, const int32_t* rec_info, const uint64_t* rec_mask,
+                              const float* rec_q, const int64_t* rec_i64, long long n_rec, int32_t* bytes, int32_t* status,
+                              void* stream) {
+    MwView V;
+    if (!mw_view(V, n_games, words, lens, log_cap, bounds, n_steps, key_steps, rec_key, rec_info, rec_mask, rec_q, rec_i64, n_rec) ||
+        !bytes || !status)
+        return fail(MJX_ERR_ARG, "mjx_mjai_render_count_dev: bad arguments");
+    V.bytes = bytes; V.status = status;
+    k_mjai_render<false><<<(n_games + MW_WARPS - 1) / MW_WARPS, MW_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+int mjx_mjai_render_fill_dev(int n_games, const uint64_t* words, const int32_t* lens, int log_cap, const int32_t* bounds,
+                             int n_steps, int key_steps, const int64_t* rec_key, const int32_t* rec_info, const uint64_t* rec_mask,
+                             const float* rec_q, const int64_t* rec_i64, long long n_rec, const int32_t* status, const int64_t* off,
+                             int g0, int g1, char* out, long long out_cap, void* stream) {
+    MwView V;
+    if (!mw_view(V, n_games, words, lens, log_cap, bounds, n_steps, key_steps, rec_key, rec_info, rec_mask, rec_q, rec_i64, n_rec) ||
+        !status || !off || g0 < 0 || g1 > n_games || g0 >= g1 || out_cap < 0 || (out_cap > 0 && !out))
+        return fail(MJX_ERR_ARG, "mjx_mjai_render_fill_dev: bad arguments");
+    V.status = const_cast<int32_t*>(status); V.off = off; V.g0 = g0; V.g1 = g1; V.out = out; V.out_cap = out_cap;
+    k_mjai_render<true><<<(g1 - g0 + MW_WARPS - 1) / MW_WARPS, MW_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
     CU(cudaGetLastError());
     return MJX_OK;
 }

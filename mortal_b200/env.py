@@ -180,6 +180,7 @@ class BatchEnv:
         _lib.check(self.L.mjx_env_enable_log(self._h, int(words_per_table)), "mjx_env_enable_log")
         self._log_cap = int(words_per_table)
         self.log_len = self._as_t(self.L.mjx_env_log_len_dev(self._h), (self.n_tables,), "<i4")  # words written so far, per table
+        self.log_words = self._as_t(self.L.mjx_env_log_words_dev(self._h), (self.n_tables, self._log_cap), "<i8")  # the words (bits)
 
     def read_log(self):
         """-> (words uint64 [n_tables, cap], lengths int32 [n_tables]); decode with mortal_b200.mjai_log"""

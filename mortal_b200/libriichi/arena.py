@@ -12,6 +12,7 @@ D2H copies of the other half run. Results are those of one batch. Device engines
 """
 from __future__ import annotations
 
+import os
 import time
 
 import numpy as np
@@ -128,7 +129,13 @@ class _Part:
         self.meta_rec = None
         if arena.log_dir is not None:
             env.enable_log()
-            self.meta_rec = _MetaRecorder(self.n, 0 if self.mixed else version) if arena.log_meta else None
+            if arena.log_meta:
+                # CUDA environments keep the records on the device (k_meta_record); others, and the host writer, use _MetaRecorder
+                from ..mjai_write import DeviceMetaRecorder
+
+                rec_version = 0 if self.mixed else version
+                self.meta_rec = (DeviceMetaRecorder(self.n, rec_version, env) if isinstance(env, BatchEnv) and not arena.host_log_writer
+                                 else _MetaRecorder(self.n, rec_version))
         self.actions = torch.zeros(env.row_cap, dtype=torch.int64, device=dev)
         guards = [bool(getattr(a, "enable_rule_based_agari_guard", False)) for a in agents]
         self.q_all = None
@@ -162,6 +169,13 @@ class _Part:
         self.first, self.cycles, self.nr = True, 0, 0
         self.recorded, self.recorded_masks = [], []
         self.mask_weights = (1 << torch.arange(46, dtype=torch.int64))
+        self.dev_meta = self.meta_rec is not None and not isinstance(self.meta_rec, _MetaRecorder)
+        if self.dev_meta and self.host_mode:  # the host engines' Q-values, greedy flags and call ids, copied to the device per cycle
+            self.h_mq, self.h_mg = pin(torch.zeros((env.row_cap, 46), dtype=torch.float32)), pin(torch.ones(env.row_cap, dtype=torch.bool))
+            self.h_mc = pin(torch.zeros(env.row_cap, dtype=torch.int32))
+            self.d_mq = torch.empty((env.row_cap, 46), dtype=torch.float32, device=dev)
+            self.d_mg = torch.empty(env.row_cap, dtype=torch.bool, device=dev)
+            self.d_mc = torch.empty(env.row_cap, dtype=torch.int32, device=dev)
 
     # every device call of the part goes to its own stream, so the two parts overlap on the GPU
     def _ctx(self):
@@ -246,14 +260,27 @@ class _Part:
                         obs_np = buf.numpy()
                     t_eval = time.perf_counter_ns()
                     a, q, greedy = agent.react_host(obs_np, self.masks_np, idx, inv_np if is_oracle else None)
-                    if meta_rec is not None:
+                    if self.dev_meta:
+                        ti = torch.from_numpy(idx)
+                        self.h_mq[ti] = torch.from_numpy(q).reshape(-1, 46)
+                        self.h_mg[ti] = torch.from_numpy(np.asarray(greedy, dtype=bool))
+                        self.h_mc[ti] = meta_rec.new_call(len(idx), time.perf_counter_ns() - t_eval)
+                    elif meta_rec is not None:
                         meta_rec.add_agent(cycles, torch.from_numpy(idx), torch.from_numpy(q).reshape(-1, 46), time.perf_counter_ns() - t_eval, greedy)
                     h_actions[torch.from_numpy(idx)] = torch.from_numpy(a)
                     if h_q is not None:
                         h_q[torch.from_numpy(idx)] = torch.from_numpy(q).reshape(-1, 46)
-                if meta_rec is not None:
-                    meta_rec.add_rows(cycles, torch.from_numpy(tbl_h).long(), torch.from_numpy(rs_h), h_actions[:nr], self.h_masks[:nr], self.h_obs[:nr])
+                if meta_rec is not None and not self.dev_meta:
+                    # a copy: h_actions is refilled every cycle, and the recorder keeps what it is given until the end
+                    meta_rec.add_rows(cycles, torch.from_numpy(tbl_h).long(), torch.from_numpy(rs_h), h_actions[:nr].clone(), self.h_masks[:nr],
+                                      self.h_obs[:nr])
                 self.actions[:nr].copy_(h_actions[:nr], non_blocking=True)
+                if self.dev_meta:  # the rows' records from the pinned buffers: three H2D copies and one k_meta_record, no host loop
+                    self.d_mq[:nr].copy_(self.h_mq[:nr], non_blocking=True)
+                    self.d_mg[:nr].copy_(self.h_mg[:nr], non_blocking=True)
+                    self.d_mc[:nr].copy_(self.h_mc[:nr], non_blocking=True)
+                    meta_rec.record(cycles, nr, self.d_mq[:nr], self.actions, greedy=self.d_mg[:nr], call_ids=self.d_mc[:nr],
+                                    obs=None if self.mixed else env.obs_buffer())
                 if h_q is not None:
                     self.q_all[:nr].copy_(h_q[:nr], non_blocking=True)
                 if self.arena.record_decisions:
@@ -279,7 +306,9 @@ class _Part:
                 self.actions[:nr] = a.to(torch.int64)
                 if self.q_all is not None:
                     self.q_all[:nr] = q.float()
-                if meta_rec is not None:
+                if self.dev_meta:
+                    meta_rec.record(cycles, nr, q, self.actions, call=meta_rec.new_call(nr, time.perf_counter_ns() - t_eval), obs=obs_buf)
+                elif meta_rec is not None:
                     meta_rec.add_agent(cycles, torch.arange(nr), q, time.perf_counter_ns() - t_eval, greedy)
             else:
                 chal = self.is_challenger[tbl % self.per, seat]
@@ -297,9 +326,12 @@ class _Part:
                     self.actions[idx] = a.to(torch.int64)
                     if self.q_all is not None:
                         self.q_all[idx] = q.float()
-                    if meta_rec is not None:
+                    if self.dev_meta:
+                        meta_rec.record(cycles, idx.numel(), q, self.actions, idx=idx,
+                                        call=meta_rec.new_call(idx.numel(), time.perf_counter_ns() - t_eval), obs=obs_buf)
+                    elif meta_rec is not None:
                         meta_rec.add_agent(cycles, idx, q, time.perf_counter_ns() - t_eval)
-            if meta_rec is not None:
+            if meta_rec is not None and not self.dev_meta:
                 meta_rec.add_rows(cycles, tbl, env.row_seat[:nr], self.actions[:nr], masks, obs)
             if self.arena.record_decisions:
                 self.recorded.append(torch.stack([tbl + self.offset, env.row_step[:nr].long(), seat, (env.row_seat[:nr] >> 2).long() & 1,
@@ -335,6 +367,8 @@ class _Arena:
         self.log_dir = log_dir  # arena/one_vs_three.rs:26-34: gz mjai logs are written here when set
         self.log_meta = True    # attach the per-decision meta (q-values, mask bits, ...) to the agent events (mortal.rs:161-186)
         self.last_meta_error = None
+        self.host_log_writer = False  # test hook: write the logs with mjai_log.write_logs even for CUDA environments
+        self.last_log_timing = None   # seconds per stage of the device log writer (count, fill_d2h, gzip_wait) of the last run
         self.record_grp = False  # keep the per-kyoku GRP features of every game (read on device, no logs): last_grp
         self.last_grp = None
         self.pipeline = True    # play the batch as two half-batches stepped alternately (see the module docstring)
@@ -401,22 +435,7 @@ class _Arena:
             results = [p.env.results() for p in parts]
             res = {k: np.concatenate([r[k] for r in results]) for k in results[0]}
             if self.log_dir is not None:  # one_vs_three.rs:195-225: one {seed}_{key}_{split}.json.gz per game
-                from .. import mjai_log
-
-                agent_names = [str(getattr(a, "name", "NoName")) for a in agents]
-                self.last_log_paths = []
-                for p in parts:
-                    words, lens = p.env.read_log()
-                    names = [[agent_names[0] if p.ic_host[g % per, seat] else agent_names[1] for seat in range(4)] for g in range(p.n)]
-                    seeds = [(int(p.nonces[g]), int(p.keys[g])) for g in range(p.n)]
-                    bounds = decisions = None
-                    if p.meta_rec is not None:
-                        try:
-                            bounds, decisions = p.meta_rec.finish()
-                        except Exception as exc:  # the logs themselves must not depend on the optional metadata
-                            self.last_meta_error = exc
-                            bounds = decisions = None
-                    self.last_log_paths += mjai_log.write_logs(self.log_dir, words, lens, seeds, names, "abcd"[:per], bounds, decisions)
+                self._write_logs(parts, agents, per)
             if self.record_grp:  # dataset/grp.rs:90-164 straight from the table records: what reward_calculator.py:13-38 consumes
                 from ..dataset import Grp
 
@@ -441,6 +460,49 @@ class _Arena:
             bad = int(np.nonzero(res["err"])[0][0])
             raise RuntimeError(f"table {bad} failed with mjx error code {int(res['err'][bad])}")
         return res
+
+    def _write_logs(self, parts, agents, per):
+        """The parts' logs, in part and game order. CUDA environments render the text on the device (mortal_b200.mjai_write) and
+        gzip on a thread pool; other environments, and parts with a game the device declines, go through mjai_log.write_logs, which
+        raises where the words are corrupt. Both write the same bytes."""
+        from concurrent.futures import ThreadPoolExecutor
+
+        from .. import mjai_log, mjai_write
+
+        agent_names = [str(getattr(a, "name", "NoName")) for a in agents]
+        self.last_log_paths = []
+        self.last_log_timing = {}
+        self.last_meta_records = sum(getattr(p.meta_rec, "count", 0) for p in parts)  # device-recorded decision rows
+        device = not self.host_log_writer and all(isinstance(p.env, BatchEnv) for p in parts)
+        pool = ThreadPoolExecutor(max_workers=os.cpu_count() or 1) if device else None
+        try:
+            for p in parts:
+                names = [[agent_names[0] if p.ic_host[g % per, seat] else agent_names[1] for seat in range(4)] for g in range(p.n)]
+                seeds = [(int(p.nonces[g]), int(p.keys[g])) for g in range(p.n)]
+                if device:
+                    dev_args = None
+                    if p.meta_rec is not None:
+                        try:
+                            dev_args = p.meta_rec.device_args()
+                        except Exception as exc:  # the logs themselves must not depend on the optional metadata
+                            self.last_meta_error = exc
+                    paths = mjai_write.write_logs_device(self.log_dir, p.env, seeds, names, "abcd"[:per], pool, timing=self.last_log_timing,
+                                                         dev_args=dev_args)
+                    if paths is not None:
+                        self.last_log_paths += paths
+                        continue
+                words, lens = p.env.read_log()
+                bounds = decisions = None
+                if p.meta_rec is not None:
+                    try:
+                        bounds, decisions = p.meta_rec.finish()
+                    except Exception as exc:  # the logs themselves must not depend on the optional metadata
+                        self.last_meta_error = exc
+                        bounds = decisions = None
+                self.last_log_paths += mjai_log.write_logs(self.log_dir, words, lens, seeds, names, "abcd"[:per], bounds, decisions)
+        finally:
+            if pool is not None:
+                pool.shutdown(wait=True)
 
     def ako_vs_py(self, *a, **k):
         raise NotImplementedError("akochan subprocess agents are out of scope (SURVEY.md §2.1 row 5)")
