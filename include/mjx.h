@@ -328,6 +328,38 @@ int mjx_grp_logs_dev(int n_logs, const uint64_t* hdr, const int32_t* ev_off, con
                      const uint8_t* has_deltas, int32_t* feat, uint8_t* rank_by_player, int64_t* final_scores, int32_t* status,
                      void* stream);
 
+/* ---- GRP training rewards: mortal/reward_calculator.py and the targets of mortal/dataloader.py:98-123 (csrc/mjx_reward.cuh) -------
+ * The per-job status: OK = the job's outputs are written; CAPACITY: the job's move range, game, player or the game's rank_by_player
+ * entry lies outside the arrays (nothing written); KYOKU: an at_kyoku lies outside [0, the game's row count) (the job's outputs are
+ * zero; the reference fails its `len(kyoku_rewards) >= at_kyoku[-1] + 1` assertion there). */
+enum mjx_reward_status { MJX_REWARD_OK = 0, MJX_REWARD_CAPACITY = 1, MJX_REWARD_KYOKU = 2 };
+/* The GRP net (model.py GRP: GRU of `layers` layers with hidden size `hidden`, Linear HL -> HL, ReLU, Linear HL -> 24, softmax,
+ * HL = hidden * layers; float64 throughout) over every prefix of every game, then the per-move training targets of every job.
+ * Device pointers unless stated.
+ *   feat         float64 [n_rows, 7]: the games' kyoku rows (Grp.take_feature()), game g's at rows [game_off[g], game_off[g + 1]);
+ *                a game whose offsets are not 0 <= lo <= hi <= n_rows has no rows (nothing written for it, its jobs CAPACITY).
+ *   weights      float64 [n_weights]: per layer k rnn.weight_ih_l{k} [3 hidden, k ? hidden : 7], rnn.weight_hh_l{k} [3 hidden,
+ *                hidden], rnn.bias_ih_l{k}, rnn.bias_hh_l{k} [3 hidden] (gates r, z, n); then fc.0.weight [HL, HL], fc.0.bias [HL],
+ *                fc.2.weight [24, HL], fc.2.bias [24]. 1 <= hidden <= 256, 1 <= layers <= 4, n_weights must match.
+ *   matrix       out float64 [n_rows, 4, 4]: row r = calc_matrix of the prefix that ends at row r: [player, rank] = the sum of the
+ *                softmax over the permutations of itertools.permutations(range(4)) that give `player` that `rank`.
+ * Jobs (n_jobs = 0: the matrix only): job j's moves are [move_off[j], move_off[j + 1]) of n_moves, of game job_game[j] (int32) and
+ * seat job_player[j] (uint8); per move at_kyoku int32, apply_gamma and dones uint8; per game rank_by_player uint8 [n_games, 4] and
+ * final_scores int64 [n_games, 4]; pts_host: 4 doubles on the host; uniform_init: row 0 of the rank probabilities is 1/4. Per move:
+ *   steps_to_done int64  0 where dones, else that of the next move + apply_gamma (the move after a job's last counts as 0);
+ *   kyoku_reward  float64 exp_pts[at_kyoku + 1] - exp_pts[at_kyoku], exp_pts[k] = [matrix[rows, player]; one_hot(final
+ *                 rank)][k] . pts;
+ *   player_rank   int64  the seat's rank in score row at_kyoku + 1 of concat(feature[:, 3:] * 1e4, [final_scores]): seats with
+ *                 a higher score plus lower-numbered seats with an equal one;
+ *   job_status    int32 [n_jobs] mjx_reward_status.
+ * Enqueued on `stream` without a synchronise; every read is bounded by n_rows, n_games and n_moves. */
+int mjx_grp_reward_dev(int n_games, const double* feat, const int32_t* game_off, long long n_rows, const double* weights,
+                       long long n_weights, int hidden, int layers, double* matrix, int n_jobs, const int32_t* move_off,
+                       long long n_moves, const int32_t* job_game, const uint8_t* job_player, const int32_t* at_kyoku,
+                       const uint8_t* apply_gamma, const uint8_t* dones, const uint8_t* rank_by_player, const int64_t* final_scores,
+                       const double* pts_host, int uniform_init, int64_t* steps_to_done, double* kyoku_reward,
+                       int64_t* player_rank, int32_t* job_status, void* stream);
+
 /* ---- libriichi.state.PlayerState (state/player_state.rs:143-264, state/getter.rs:6-156, state/obs_repr.rs:776-791) ---------
  * A batch of n independent single-seat states: table records in single-seat mode (other seats' hidden tiles are `?` = 37), updated
  * by the same device event handlers self-play uses. `mjx_state_create` returns an mjx_env whose encoder entry points

@@ -14,6 +14,7 @@
 #include "mjx_mjai_write.cuh"
 #include "mjx_stat.cuh"
 #include "mjx_grp.cuh"
+#include "mjx_reward.cuh"
 #include "mjx_invisible.cuh"
 #include "mjx_state.cuh"
 #include "mjx_nn.cuh"
@@ -1620,6 +1621,38 @@ int mjx_grp_logs_dev(int n_logs, const uint64_t* hdr, const int32_t* ev_off, con
     V.n_kyoku = n_kyoku_words / REPLAY_KYOKU_WORDS; V.deltas = deltas; V.has_deltas = has_deltas; V.n_logs = n_logs;
     V.feat = feat; V.rank = rank_by_player; V.final = final_scores; V.status = status;
     k_grp_logs<<<(n_logs + GRP_WARPS - 1) / GRP_WARPS, GRP_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+// ---- GRP training rewards (reward_calculator.py, dataloader.py:98-123)
+int mjx_grp_reward_dev(int n_games, const double* feat, const int32_t* game_off, long long n_rows, const double* weights,
+                       long long n_weights, int hidden, int layers, double* matrix, int n_jobs, const int32_t* move_off,
+                       long long n_moves, const int32_t* job_game, const uint8_t* job_player, const int32_t* at_kyoku,
+                       const uint8_t* apply_gamma, const uint8_t* dones, const uint8_t* rank_by_player, const int64_t* final_scores,
+                       const double* pts_host, int uniform_init, int64_t* steps_to_done, double* kyoku_reward,
+                       int64_t* player_rank, int32_t* job_status, void* stream) {
+    if (rw_check_args(n_games, feat, game_off, n_rows, weights, n_weights, hidden, layers, matrix, n_jobs, move_off, n_moves, job_game,
+                      job_player, at_kyoku, apply_gamma, dones, rank_by_player, final_scores, pts_host, steps_to_done, kyoku_reward,
+                      player_rank, job_status))
+        return fail(MJX_ERR_ARG, "mjx_grp_reward_dev: bad arguments");
+    const cudaStream_t st = (cudaStream_t)stream;
+    MatrixView M;
+    M.feat = feat; M.game_off = game_off; M.n_rows = n_rows; M.n_games = n_games; M.net = GrpNet{weights, hidden, layers};
+    M.matrix = matrix;
+    const int smem = rw_smem_doubles(hidden, layers) * (int)sizeof(double);
+    if (smem > 48 * 1024) CU(cudaFuncSetAttribute(k_grp_matrix, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    k_grp_matrix<<<(n_games + RW_GAMES - 1) / RW_GAMES, RW_THREADS, smem, st>>>(M);
+    CU(cudaGetLastError());
+    if (n_jobs == 0) return MJX_OK;
+    TargetView T;
+    T.feat = feat; T.game_off = game_off; T.n_rows = n_rows; T.n_games = n_games; T.matrix = matrix;
+    T.rank_by_player = rank_by_player; T.final_scores = final_scores; T.uniform_init = uniform_init != 0;
+    for (int k = 0; k < 4; k++) T.pts[k] = pts_host[k];
+    T.move_off = move_off; T.n_moves = n_moves; T.job_game = job_game; T.job_player = job_player; T.n_jobs = n_jobs;
+    T.at_kyoku = at_kyoku; T.apply_gamma = apply_gamma; T.dones = dones;
+    T.steps_to_done = steps_to_done; T.kyoku_reward = kyoku_reward; T.player_rank = player_rank; T.status = job_status;
+    k_train_targets<<<(n_jobs + RW_WARPS - 1) / RW_WARPS, RW_WARPS * 32, 0, st>>>(T);
     CU(cudaGetLastError());
     return MJX_OK;
 }
