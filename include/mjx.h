@@ -434,7 +434,9 @@ int mjx_env_policy_test(mjx_env* env, int kind, int64_t* actions_dev, int64_t* t
 
 /* ---- policy-net inference helpers (not part of libriichi's surface; mortal/model.py ResBlock + ChannelAttention) ------------
  * Fused elementwise passes between the cuDNN convolutions: bf16 channels-last activations [batch, length, channels]
- * (device pointers, 16-byte aligned, channels % 8 == 0), fp32 math. scale/bias = eval-mode BatchNorm folded to an affine. */
+ * (device pointers, 16-byte aligned, channels % 8 == 0), fp32 math. scale/bias = eval-mode BatchNorm folded to an affine.
+ * Every array pointer (activations, gate, scale / bias, w1 / b1 / w2t / b2) must be 16-byte aligned; a misaligned one fails the
+ * call with MJX_ERR_ARG before anything is launched (obs_to_nhwc: `out` 16-byte, `obs` float aligned). */
 int mjx_nn_affine_mish_bf16(const void* x, const float* scale, const float* bias, void* out, long long n_elems, int channels,
                             void* stream);                                   /* out = mish(x * scale[c] + bias[c]) */
 int mjx_nn_pool_bf16(const void* x, void* avg, void* mx, int batch, int length, int channels, void* stream);  /* [batch, channels] each */

@@ -1,6 +1,8 @@
 // mortal_b200 — CUDA kernels (sm_90a) and the C ABI of include/mjx.h.
+#include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -1928,10 +1930,17 @@ static int nn_grid_for(size_t n_items, int c8) {
     const int g = nn_grid(n_items);
     return (g + unit - 1) / unit * unit;
 }
+// the kernels read activations as 16-byte Vec8 and scale / bias / w1 / w2t as float4: a misaligned pointer (a view at an odd
+// offset into a larger buffer) would fault on the device, so it is refused with the other argument checks
+static bool nn_misaligned(std::initializer_list<const void*> ps) {
+    for (const void* p : ps)
+        if ((uintptr_t)p % 16) return true;
+    return false;
+}
 int mjx_nn_affine_mish_bf16(const void* x, const float* scale, const float* bias, void* out, long long n_elems, int channels,
                             void* stream) {
-    if (!x || !scale || !bias || !out || channels <= 0 || channels % 8 || n_elems % channels)
-        return fail(MJX_ERR_ARG, "mjx_nn_affine_mish_bf16: bad arguments");
+    if (!x || !scale || !bias || !out || channels <= 0 || channels % 8 || n_elems % channels || nn_misaligned({x, scale, bias, out}))
+        return fail(MJX_ERR_ARG, "mjx_nn_affine_mish_bf16: bad arguments (pointers 16-byte aligned)");
     if (!g_ready) return fail(MJX_ERR_STATE, "mjx_nn_*: call mjx_init first");
     const size_t n_vec = (size_t)n_elems / 8;
     mjx_nn::k_affine_mish<<<nn_grid_for(n_vec, channels / 8), 256, 0, (cudaStream_t)stream>>>((const mjx_nn::Vec8*)x, scale, bias, (mjx_nn::Vec8*)out,
@@ -1940,8 +1949,8 @@ int mjx_nn_affine_mish_bf16(const void* x, const float* scale, const float* bias
     return MJX_OK;
 }
 int mjx_nn_pool_bf16(const void* x, void* avg, void* mx, int batch, int length, int channels, void* stream) {
-    if (!x || !avg || !mx || batch <= 0 || length <= 0 || channels <= 0 || channels % 8)
-        return fail(MJX_ERR_ARG, "mjx_nn_pool_bf16: bad arguments");
+    if (!x || !avg || !mx || batch <= 0 || length <= 0 || channels <= 0 || channels % 8 || nn_misaligned({x, avg, mx}))
+        return fail(MJX_ERR_ARG, "mjx_nn_pool_bf16: bad arguments (pointers 16-byte aligned)");
     if (!g_ready) return fail(MJX_ERR_STATE, "mjx_nn_*: call mjx_init first");
     mjx_nn::k_pool<<<nn_grid((size_t)batch * (channels / 8)), 256, 0, (cudaStream_t)stream>>>(
         (const mjx_nn::Vec8*)x, (mjx_nn::Vec8*)avg, (mjx_nn::Vec8*)mx, batch, length, channels / 8);
@@ -1950,8 +1959,9 @@ int mjx_nn_pool_bf16(const void* x, void* avg, void* mx, int batch, int length, 
 }
 int mjx_nn_obs_to_nhwc_bf16(const float* obs, void* out, int batch, int channels, int length, int channels_padded, void* stream) {
     if (!obs || !out || batch <= 0 || channels <= 0 || length <= 0 || length > 128 || channels_padded < channels ||
-        channels_padded % mjx_nn::NHWC_TC)
-        return fail(MJX_ERR_ARG, "mjx_nn_obs_to_nhwc_bf16: bad arguments (channels_padded a multiple of 64, length <= 128)");
+        channels_padded % mjx_nn::NHWC_TC || (uintptr_t)obs % sizeof(float) || nn_misaligned({out}))
+        return fail(MJX_ERR_ARG, "mjx_nn_obs_to_nhwc_bf16: bad arguments (channels_padded a multiple of 64, length <= 128, out "
+                                 "16-byte aligned)");
     if (!g_ready) return fail(MJX_ERR_STATE, "mjx_nn_*: call mjx_init first");
     const size_t smem = (size_t)mjx_nn::NHWC_TC * (length + 1) * sizeof(float);
     const long long grid = (long long)batch * (channels_padded / mjx_nn::NHWC_TC);
@@ -1964,8 +1974,10 @@ int mjx_nn_block_tail_bf16(const void* y, const void* x, const float* w1, const 
                            const float* scale, const float* bias, void* gate_scratch, void* x_out, void* a_out, int batch, int length,
                            int channels, int hidden, void* stream) {
     if (!y || !x || !w1 || !b1 || !w2t || !b2 || !scale || !bias || !gate_scratch || !x_out || !a_out || batch <= 0 || length <= 0 ||
-        channels <= 0 || channels % 8 || channels > 256 || hidden <= 0 || hidden > 64)
-        return fail(MJX_ERR_ARG, "mjx_nn_block_tail_bf16: bad arguments (channels % 8 == 0, <= 256; hidden <= 64)");
+        channels <= 0 || channels % 8 || channels > 256 || hidden <= 0 || hidden > 64 ||
+        nn_misaligned({y, x, w1, b1, w2t, b2, scale, bias, gate_scratch, x_out, a_out}))
+        return fail(MJX_ERR_ARG, "mjx_nn_block_tail_bf16: bad arguments (channels % 8 == 0, <= 256; hidden <= 64; pointers 16-byte "
+                                 "aligned)");
     if (!g_ready) return fail(MJX_ERR_STATE, "mjx_nn_*: call mjx_init first");
     cudaStream_t st = (cudaStream_t)stream;
     const int c8 = channels / 8;
@@ -1983,8 +1995,8 @@ int mjx_nn_block_tail_bf16(const void* y, const void* x, const float* w1, const 
 }
 int mjx_nn_gate_residual_bf16(const void* y, const void* gate, const void* x, void* out, int batch, int length, int channels,
                               void* stream) {
-    if (!y || !gate || !x || !out || batch <= 0 || length <= 0 || channels <= 0 || channels % 8)
-        return fail(MJX_ERR_ARG, "mjx_nn_gate_residual_bf16: bad arguments");
+    if (!y || !gate || !x || !out || batch <= 0 || length <= 0 || channels <= 0 || channels % 8 || nn_misaligned({y, gate, x, out}))
+        return fail(MJX_ERR_ARG, "mjx_nn_gate_residual_bf16: bad arguments (pointers 16-byte aligned)");
     if (!g_ready) return fail(MJX_ERR_STATE, "mjx_nn_*: call mjx_init first");
     const size_t n_vec = (size_t)batch * length * (channels / 8);
     mjx_nn::k_gate_residual<<<nn_grid(n_vec), 256, 0, (cudaStream_t)stream>>>((const mjx_nn::Vec8*)y, (const mjx_nn::Vec8*)gate,

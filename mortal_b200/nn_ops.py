@@ -1,5 +1,6 @@
 """ctypes wrappers of the fused policy-net kernels in libmjx (csrc/mjx_nn.cuh). Tensors are CUDA bf16, logically
-[B, C, 1, L] in channels_last memory format, i.e. [B, L, C] in memory."""
+[B, C, 1, L] in channels_last memory format, i.e. [B, L, C] in memory. Every tensor handed to a kernel must start on a
+16-byte boundary (the kernels read 16-byte vectors): a view at an odd offset into a larger buffer is refused here."""
 from __future__ import annotations
 
 import ctypes as C
@@ -13,10 +14,16 @@ def _stream(t: torch.Tensor):
     return C.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
 
 
+def _aligned(*ts: torch.Tensor):
+    for t in ts:
+        assert t.is_cuda and t.data_ptr() % 16 == 0, "nn_ops: tensors must be CUDA and 16-byte aligned"
+
+
 def _check_nhwc(x: torch.Tensor):
     assert x.is_cuda and x.dtype == torch.bfloat16 and x.dim() == 4 and x.shape[2] == 1
     b, c, _, l = x.shape
     assert c % 8 == 0 and x.stride(1) == 1 and x.stride(3) == c and x.stride(0) == c * l, "expected channels_last [B, C, 1, L]"
+    _aligned(x)
     return b, c, l
 
 
@@ -24,6 +31,8 @@ def affine_mish(x: torch.Tensor, scale: torch.Tensor, bias: torch.Tensor) -> tor
     """mish(x * scale[c] + bias[c]); scale / bias float32 [C]"""
     b, c, l = _check_nhwc(x)
     assert scale.dtype == torch.float32 and bias.dtype == torch.float32 and scale.numel() == c == bias.numel()
+    assert scale.is_contiguous() and bias.is_contiguous()
+    _aligned(scale, bias)
     out = torch.empty_like(x)
     _lib.check(_lib.load().mjx_nn_affine_mish_bf16(C.c_void_p(x.data_ptr()), C.c_void_p(scale.data_ptr()), C.c_void_p(bias.data_ptr()),
                                                    C.c_void_p(out.data_ptr()), x.numel(), c, _stream(x)), "mjx_nn_affine_mish_bf16")
@@ -44,6 +53,7 @@ def gate_residual(y: torch.Tensor, gate: torch.Tensor, x: torch.Tensor) -> torch
     """y * gate[b, c] + x; gate bf16 [B, C] contiguous"""
     b, c, l = _check_nhwc(y)
     assert _check_nhwc(x) == (b, c, l) and gate.dtype == torch.bfloat16 and gate.shape == (b, c) and gate.is_contiguous()
+    _aligned(gate)
     out = torch.empty_like(y)
     _lib.check(_lib.load().mjx_nn_gate_residual_bf16(C.c_void_p(y.data_ptr()), C.c_void_p(gate.data_ptr()), C.c_void_p(x.data_ptr()),
                                                      C.c_void_p(out.data_ptr()), b, l, c, _stream(y)), "mjx_nn_gate_residual_bf16")
@@ -59,6 +69,7 @@ def block_tail(y: torch.Tensor, x: torch.Tensor, w1: torch.Tensor, b1: torch.Ten
     h = w1.shape[0]
     for t, shape in ((w1, (h, c)), (b1, (h,)), (w2t, (h, c)), (b2, (c,)), (scale, (c,)), (bias, (c,))):
         assert t.dtype == torch.float32 and tuple(t.shape) == shape and t.is_contiguous() and t.is_cuda
+    _aligned(w1, b1, w2t, b2, scale, bias)
     assert c <= 256, "block_tail: at most 256 channels"
     x_out, a_out = torch.empty_like(y), torch.empty_like(y)
     gate = torch.empty((b, c), dtype=torch.bfloat16, device=y.device)
