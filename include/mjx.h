@@ -454,6 +454,22 @@ int mjx_nn_block_tail_bf16(const void* y, const void* x, const float* w1, const 
                            const float* scale, const float* bias, void* gate_scratch /* bf16 [batch, channels] */, void* x_out,
                            void* a_out, int batch, int length, int channels, int hidden, void* stream);
 
+/* Version 1 (post-activation ResNet, mortal/model.py ResBlock with pre_actv=False) and oracle brains:
+ * out = relu(x * scale[c] + bias[c]): the stem's BatchNorm + ReLU and each block's first BatchNorm + ReLU. */
+int mjx_nn_affine_relu_bf16(const void* x, const float* scale, const float* bias, void* out, long long n_elems, int channels,
+                            void* stream);
+/* The post-activation block's tail, y = conv2 output: t = y * scale[c] + bias[c] (the block's second BatchNorm, fp32);
+ * gate = sigmoid(mlp(mean_l t) + mlp(max_l t)), mlp = w2 . relu(w1 . v + b1) + b2 (w2 TRANSPOSED as w2t [hidden, channels]);
+ * x_out = relu(t * gate + x). Two launches, as mjx_nn_block_tail_bf16. channels % 8 == 0, <= 256; hidden <= 64. */
+int mjx_nn_post_block_tail_bf16(const void* y, const void* x, const float* scale, const float* bias, const float* w1, const float* b1,
+                                const float* w2t, const float* b2, void* gate_scratch /* bf16 [batch, channels] */, void* x_out,
+                                int batch, int length, int channels, int hidden, void* stream);
+/* The oracle stem input: obs f32 [batch, channels, length] and obs2 (the invisible observation) f32 [batch, channels2, length] ->
+ * bf16 channels-last [batch, length, channels_padded]: channels [0, channels) from obs, then channels2 from obs2, then zeros
+ * (channels_padded % 64 == 0, >= channels + channels2). obs / obs2 float aligned, out 16-byte aligned. */
+int mjx_nn_obs2_to_nhwc_bf16(const float* obs, const float* obs2, void* out, int batch, int channels, int channels2, int length,
+                             int channels_padded, void* stream);
+
 /* ---- standalone kernels (BASELINE configs 3/4) ------------------------------------------------ */
 /* algo/shanten.rs:138-150 calc_all: tiles_dev uint8 [n,34], len_div3_dev uint8 [n] -> int8 [n]. */
 int mjx_shanten(const uint8_t* tiles_dev, const uint8_t* len_div3_dev, int8_t* out_dev, int n, void* stream);

@@ -78,6 +78,9 @@ SYMBOLS = {
     "mjx_nn_gate_residual_bf16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "mjx_nn_obs_to_nhwc_bf16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "mjx_nn_block_tail_bf16": (C.c_int, [C.c_void_p] * 11 + [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "mjx_nn_affine_relu_bf16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_void_p]),
+    "mjx_nn_post_block_tail_bf16": (C.c_int, [C.c_void_p] * 10 + [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "mjx_nn_obs2_to_nhwc_bf16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int] * 5 + [C.c_void_p]),
     "mjx_env_create_replay": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p,
                                         C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_int]),
     "mjx_env_create_replay_dev": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong,

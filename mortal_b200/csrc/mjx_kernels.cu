@@ -1948,6 +1948,17 @@ int mjx_nn_affine_mish_bf16(const void* x, const float* scale, const float* bias
     CU(cudaGetLastError());
     return MJX_OK;
 }
+int mjx_nn_affine_relu_bf16(const void* x, const float* scale, const float* bias, void* out, long long n_elems, int channels,
+                            void* stream) {
+    if (!x || !scale || !bias || !out || channels <= 0 || channels % 8 || n_elems % channels || nn_misaligned({x, scale, bias, out}))
+        return fail(MJX_ERR_ARG, "mjx_nn_affine_relu_bf16: bad arguments (pointers 16-byte aligned)");
+    if (!g_ready) return fail(MJX_ERR_STATE, "mjx_nn_*: call mjx_init first");
+    const size_t n_vec = (size_t)n_elems / 8;
+    mjx_nn::k_affine_relu<<<nn_grid_for(n_vec, channels / 8), 256, 0, (cudaStream_t)stream>>>((const mjx_nn::Vec8*)x, scale, bias, (mjx_nn::Vec8*)out,
+                                                                            n_vec, channels / 8);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
 int mjx_nn_pool_bf16(const void* x, void* avg, void* mx, int batch, int length, int channels, void* stream) {
     if (!x || !avg || !mx || batch <= 0 || length <= 0 || channels <= 0 || channels % 8 || nn_misaligned({x, avg, mx}))
         return fail(MJX_ERR_ARG, "mjx_nn_pool_bf16: bad arguments (pointers 16-byte aligned)");
@@ -1967,6 +1978,22 @@ int mjx_nn_obs_to_nhwc_bf16(const float* obs, void* out, int batch, int channels
     const long long grid = (long long)batch * (channels_padded / mjx_nn::NHWC_TC);
     if (grid > 0x7fffffffLL) return fail(MJX_ERR_ARG, "mjx_nn_obs_to_nhwc_bf16: batch too large");
     mjx_nn::k_obs_to_nhwc<<<(int)grid, 256, smem, (cudaStream_t)stream>>>(obs, (__nv_bfloat16*)out, channels, length, channels_padded);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+int mjx_nn_obs2_to_nhwc_bf16(const float* obs, const float* obs2, void* out, int batch, int channels, int channels2, int length,
+                             int channels_padded, void* stream) {
+    if (!obs || !obs2 || !out || batch <= 0 || channels <= 0 || channels2 <= 0 || length <= 0 || length > 128 ||
+        channels_padded < channels + channels2 || channels_padded % mjx_nn::NHWC_TC || (uintptr_t)obs % sizeof(float) ||
+        (uintptr_t)obs2 % sizeof(float) || nn_misaligned({out}))
+        return fail(MJX_ERR_ARG, "mjx_nn_obs2_to_nhwc_bf16: bad arguments (channels_padded >= channels + channels2 and a multiple of "
+                                 "64, length <= 128, out 16-byte aligned)");
+    if (!g_ready) return fail(MJX_ERR_STATE, "mjx_nn_*: call mjx_init first");
+    const size_t smem = (size_t)mjx_nn::NHWC_TC * (length + 1) * sizeof(float);
+    const long long grid = (long long)batch * (channels_padded / mjx_nn::NHWC_TC);
+    if (grid > 0x7fffffffLL) return fail(MJX_ERR_ARG, "mjx_nn_obs2_to_nhwc_bf16: batch too large");
+    mjx_nn::k_obs2_to_nhwc<<<(int)grid, 256, smem, (cudaStream_t)stream>>>(obs, obs2, (__nv_bfloat16*)out, channels, channels2, length,
+                                                                           channels_padded);
     CU(cudaGetLastError());
     return MJX_OK;
 }
@@ -1990,6 +2017,29 @@ int mjx_nn_block_tail_bf16(const void* y, const void* x, const float* w1, const 
     mjx_nn::k_gate_residual_mish<<<nn_grid_for(n_vec, c8), 256, 0, st>>>(
         (const mjx_nn::Vec8*)y, (const mjx_nn::Vec8*)gate_scratch, (const mjx_nn::Vec8*)x, scale, bias, (mjx_nn::Vec8*)x_out,
         (mjx_nn::Vec8*)a_out, n_vec, length, c8);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+int mjx_nn_post_block_tail_bf16(const void* y, const void* x, const float* scale, const float* bias, const float* w1, const float* b1,
+                                const float* w2t, const float* b2, void* gate_scratch, void* x_out, int batch, int length, int channels,
+                                int hidden, void* stream) {
+    if (!y || !x || !scale || !bias || !w1 || !b1 || !w2t || !b2 || !gate_scratch || !x_out || batch <= 0 || length <= 0 ||
+        channels <= 0 || channels % 8 || channels > 256 || hidden <= 0 || hidden > 64 ||
+        nn_misaligned({y, x, scale, bias, w1, b1, w2t, b2, gate_scratch, x_out}))
+        return fail(MJX_ERR_ARG, "mjx_nn_post_block_tail_bf16: bad arguments (channels % 8 == 0, <= 256; hidden <= 64; pointers "
+                                 "16-byte aligned)");
+    if (!g_ready) return fail(MJX_ERR_STATE, "mjx_nn_*: call mjx_init first");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int c8 = channels / 8;
+    const int warps_per_cta = 8;
+    const int grid = std::max(1, std::min((batch + warps_per_cta - 1) / warps_per_cta, g_sm_count * 8));
+    mjx_nn::k_pool_gate_affine_relu<<<grid, warps_per_cta * 32, 0, st>>>((const mjx_nn::Vec8*)y, scale, bias, w1, b1, w2t, b2,
+                                                                           (mjx_nn::Vec8*)gate_scratch, batch, length, c8, hidden);
+    CU(cudaGetLastError());
+    const size_t n_vec = (size_t)batch * length * c8;
+    mjx_nn::k_affine_gate_residual_relu<<<nn_grid_for(n_vec, c8), 256, 0, st>>>(
+        (const mjx_nn::Vec8*)y, (const mjx_nn::Vec8*)gate_scratch, (const mjx_nn::Vec8*)x, scale, bias, (mjx_nn::Vec8*)x_out, n_vec,
+        length, c8);
     CU(cudaGetLastError());
     return MJX_OK;
 }

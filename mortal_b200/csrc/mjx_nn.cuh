@@ -37,28 +37,45 @@ __device__ __forceinline__ Affine8 load_affine8(const float* __restrict__ scale,
     a.b[0] = b0.x; a.b[1] = b0.y; a.b[2] = b0.z; a.b[3] = b0.w; a.b[4] = b1.x; a.b[5] = b1.y; a.b[6] = b1.z; a.b[7] = b1.w;
     return a;
 }
-__device__ __forceinline__ Vec8 affine_mish8(const Vec8& in, const Affine8& A) {
+// the activations the kernels are instantiated with: Mish (versions 2-4) and ReLU (version 1, mortal/model.py:120-130). ReLU
+// keeps a NaN, as torch.relu does (fmaxf would turn it into 0).
+__device__ __forceinline__ float relu_f(float x) { return x < 0.f ? 0.f : x; }
+struct MishAct { __device__ __forceinline__ static float f(float x) { return mish_f(x); } };
+struct ReluAct { __device__ __forceinline__ static float f(float x) { return relu_f(x); } };
+
+template <class Act>
+__device__ __forceinline__ Vec8 affine_act8(const Vec8& in, const Affine8& A) {
     Vec8 o;
 #pragma unroll
     for (int k = 0; k < 4; k++) {
         const float2 f = __bfloat1622float2(in.v[k]);
-        o.v[k] = __floats2bfloat162_rn(mish_f(fmaf(f.x, A.s[2 * k], A.b[2 * k])), mish_f(fmaf(f.y, A.s[2 * k + 1], A.b[2 * k + 1])));
+        o.v[k] = __floats2bfloat162_rn(Act::f(fmaf(f.x, A.s[2 * k], A.b[2 * k])), Act::f(fmaf(f.y, A.s[2 * k + 1], A.b[2 * k + 1])));
     }
     return o;
 }
+__device__ __forceinline__ Vec8 affine_mish8(const Vec8& in, const Affine8& A) { return affine_act8<MishAct>(in, A); }
 
-// out = mish(x * scale[c] + bias[c]); gridDim.x * blockDim.x is a multiple of c8
-__global__ void __launch_bounds__(256) k_affine_mish(const Vec8* __restrict__ x, const float* __restrict__ scale,
-                                                     const float* __restrict__ bias, Vec8* __restrict__ out, size_t n_vec, int c8) {
+// out = act(x * scale[c] + bias[c]); gridDim.x * blockDim.x is a multiple of c8
+template <class Act>
+__device__ __forceinline__ void affine_act_pass(const Vec8* __restrict__ x, const float* __restrict__ scale, const float* __restrict__ bias,
+                                                Vec8* __restrict__ out, size_t n_vec, int c8) {
     const size_t t0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
     const Affine8 A = load_affine8(scale, bias, (int)(t0 % (size_t)c8));
     size_t v = t0;
     for (; v + stride < n_vec; v += 2 * stride) {  // two independent vectors in flight per thread
         const Vec8 i0 = x[v], i1 = x[v + stride];
-        out[v] = affine_mish8(i0, A);
-        out[v + stride] = affine_mish8(i1, A);
+        out[v] = affine_act8<Act>(i0, A);
+        out[v + stride] = affine_act8<Act>(i1, A);
     }
-    if (v < n_vec) out[v] = affine_mish8(x[v], A);
+    if (v < n_vec) out[v] = affine_act8<Act>(x[v], A);
+}
+__global__ void __launch_bounds__(256) k_affine_mish(const Vec8* __restrict__ x, const float* __restrict__ scale,
+                                                     const float* __restrict__ bias, Vec8* __restrict__ out, size_t n_vec, int c8) {
+    affine_act_pass<MishAct>(x, scale, bias, out, n_vec, c8);
+}
+__global__ void __launch_bounds__(256) k_affine_relu(const Vec8* __restrict__ x, const float* __restrict__ scale,
+                                                     const float* __restrict__ bias, Vec8* __restrict__ out, size_t n_vec, int c8) {
+    affine_act_pass<ReluAct>(x, scale, bias, out, n_vec, c8);
 }
 
 // avg[b, c] = mean_l x[b, l, c], mx[b, c] = max_l x[b, l, c]   (ChannelAttention pooling)
@@ -117,14 +134,21 @@ __global__ void __launch_bounds__(256) k_gate_residual(const Vec8* __restrict__ 
 // lanes past c8 idle), a position is c8 consecutive 16-byte loads of the warp and eight positions are in flight per lane; the MLP
 // weights (w1 [H][C] and w2 TRANSPOSED to [H][C], 2 x 9 KB at C = 192) are read through L1 as two float4 per lane and use.
 // fp32 throughout (the bf16 pipeline this replaces rounded the pooled vectors, the hidden layer and the logits); the gate is stored as bf16.
-__global__ void __launch_bounds__(256) k_pool_gate(const Vec8* __restrict__ y, const float* __restrict__ w1, const float* __restrict__ b1,
-                                                   const float* __restrict__ w2t, const float* __restrict__ b2, Vec8* __restrict__ gate,
-                                                   int batch, int length, int c8, int hidden) {
+// Act is the MLP's hidden activation. kAffine: the pooled values are y * scale[c] + bias[c] in fp32 (the post-activation block's
+// second BatchNorm, which sits between the convolution and the attention): applied to every element BEFORE the pooling, because a
+// negative scale turns the max of y into the max of the affine's minimum.
+template <class Act, bool kAffine>
+__device__ __forceinline__ void pool_gate_rows(const Vec8* __restrict__ y, const float* __restrict__ scale, const float* __restrict__ bias,
+                                               const float* __restrict__ w1, const float* __restrict__ b1, const float* __restrict__ w2t,
+                                               const float* __restrict__ b2, Vec8* __restrict__ gate, int batch, int length, int c8,
+                                               int hidden) {
     const int C = c8 * 8;
     const int lane = threadIdx.x & 31, warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
     const bool act = lane < c8;
     const int cv = act ? lane : 0;
     const float inv_len = 1.f / (float)length;
+    Affine8 A;
+    if constexpr (kAffine) A = load_affine8(scale, bias, cv);
     for (int b = warp; b < batch; b += nwarps) {
         const Vec8* row = y + (size_t)b * length * c8 + cv;
         float s[8], m[8];
@@ -136,7 +160,8 @@ __global__ void __launch_bounds__(256) k_pool_gate(const Vec8* __restrict__ y, c
                 const Vec8 in = row[(size_t)l * c8];
 #pragma unroll
                 for (int k = 0; k < 4; k++) {
-                    const float2 f = __bfloat1622float2(in.v[k]);
+                    float2 f = __bfloat1622float2(in.v[k]);
+                    if constexpr (kAffine) { f.x = fmaf(f.x, A.s[2 * k], A.b[2 * k]); f.y = fmaf(f.y, A.s[2 * k + 1], A.b[2 * k + 1]); }
                     s[2 * k] += f.x; s[2 * k + 1] += f.y;
                     m[2 * k] = fmaxf(m[2 * k], f.x); m[2 * k + 1] = fmaxf(m[2 * k + 1], f.y);
                 }
@@ -157,7 +182,7 @@ __global__ void __launch_bounds__(256) k_pool_gate(const Vec8* __restrict__ y, c
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) { pa += __shfl_xor_sync(0xffffffffu, pa, o); pm += __shfl_xor_sync(0xffffffffu, pm, o); }
             const float bj = __ldg(b1 + j);
-            const float ha = mish_f(pa + bj), hm = mish_f(pm + bj);
+            const float ha = Act::f(pa + bj), hm = Act::f(pm + bj);
 #pragma unroll
             for (int k = 0; k < 8; k++) { oa[k] = fmaf(vj[k], ha, oa[k]); om[k] = fmaf(vj[k], hm, om[k]); }
         }
@@ -171,6 +196,20 @@ __global__ void __launch_bounds__(256) k_pool_gate(const Vec8* __restrict__ y, c
             gate[(size_t)b * c8 + cv] = g;
         }
     }
+}
+// the pre-activation block's attention (versions 2-4): Mish hidden layer, pooling of y itself
+__global__ void __launch_bounds__(256) k_pool_gate(const Vec8* __restrict__ y, const float* __restrict__ w1, const float* __restrict__ b1,
+                                                   const float* __restrict__ w2t, const float* __restrict__ b2, Vec8* __restrict__ gate,
+                                                   int batch, int length, int c8, int hidden) {
+    pool_gate_rows<MishAct, false>(y, nullptr, nullptr, w1, b1, w2t, b2, gate, batch, length, c8, hidden);
+}
+// the post-activation block's attention (version 1): ReLU hidden layer, pooling of y * scale + bias
+__global__ void __launch_bounds__(256) k_pool_gate_affine_relu(const Vec8* __restrict__ y, const float* __restrict__ scale,
+                                                               const float* __restrict__ bias, const float* __restrict__ w1,
+                                                               const float* __restrict__ b1, const float* __restrict__ w2t,
+                                                               const float* __restrict__ b2, Vec8* __restrict__ gate, int batch, int length,
+                                                               int c8, int hidden) {
+    pool_gate_rows<ReluAct, true>(y, scale, bias, w1, b1, w2t, b2, gate, batch, length, c8, hidden);
 }
 
 // x_out = y * gate[b, c] + x and a_out = mish(x_out * scale[c] + bias[c]) (the next block's pre-activation) in one streaming pass;
@@ -195,22 +234,61 @@ __global__ void __launch_bounds__(256) k_gate_residual_mish(const Vec8* __restri
     }
 }
 
+// The post-activation block's tail (version 1: conv2 -> BN -> attention -> + x -> ReLU) as one streaming pass:
+// x_out = relu((y * scale[c] + bias[c]) * gate[b, c] + x), the BN affine in fp32 (not folded into conv2's bf16 weights);
+// gridDim.x * blockDim.x is a multiple of c8 (see k_affine_mish)
+__global__ void __launch_bounds__(256) k_affine_gate_residual_relu(const Vec8* __restrict__ y, const Vec8* __restrict__ gate,
+                                                                   const Vec8* __restrict__ x, const float* __restrict__ scale,
+                                                                   const float* __restrict__ bias, Vec8* __restrict__ x_out, size_t n_vec,
+                                                                   int length, int c8) {
+    const size_t t0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
+    const int cv = (int)(t0 % (size_t)c8);
+    const Affine8 A = load_affine8(scale, bias, cv);
+    const size_t per_b = (size_t)length * c8;
+    for (size_t v = t0; v < n_vec; v += stride) {
+        const Vec8 yy = y[v], xx = x[v], g = gate[(v / per_b) * c8 + cv];
+        Vec8 xo;
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const float2 fy = __bfloat1622float2(yy.v[k]), fx = __bfloat1622float2(xx.v[k]), fg = __bfloat1622float2(g.v[k]);
+            const float u0 = fmaf(fy.x, A.s[2 * k], A.b[2 * k]), u1 = fmaf(fy.y, A.s[2 * k + 1], A.b[2 * k + 1]);
+            xo.v[k] = __floats2bfloat162_rn(relu_f(fmaf(u0, fg.x, fx.x)), relu_f(fmaf(u1, fg.y, fx.y)));
+        }
+        x_out[v] = xo;
+    }
+}
+
 // The network's first step as one pass: observations f32 [batch, channels, length] (libriichi's layout: one row of `length` floats
 // per channel) -> bf16 channels-last [batch, length, cpad] with the channel count padded with zeros to a multiple of 64, which is
 // what the stem convolution's implicit GEMM wants (PyTorch + cuDNN otherwise run a cast, a layout copy and two padding kernels).
 // One CTA = 64 channels of one observation through a shared-memory tile.
 constexpr int NHWC_TC = 64;
-__global__ void __launch_bounds__(256) k_obs_to_nhwc(const float* __restrict__ obs, __nv_bfloat16* __restrict__ out, int channels, int length,
-                                                     int cpad) {
+// kTwo: the oracle brains' input (mortal/model.py Brain.forward: torch.cat((obs, invisible_obs), dim=1)) read from its two sources
+// without the concatenation: channels [0, c1) from obs [batch, c1, length], [c1, c1 + c2) from obs2 [batch, c2, length]. A chunk may
+// straddle the boundary; each of its two parts is contiguous in its source.
+template <bool kTwo>
+__device__ __forceinline__ void obs_chunk_to_nhwc(const float* __restrict__ obs, const float* __restrict__ obs2, __nv_bfloat16* __restrict__ out,
+                                                  int c1, int c2, int length, int cpad) {
     extern __shared__ float tile[];  // [NHWC_TC][length + 1]
+    const int channels = kTwo ? c1 + c2 : c1;
     const int chunks = cpad / NHWC_TC;
     const int b = blockIdx.x / chunks, c0 = (blockIdx.x - b * chunks) * NHWC_TC;
     const int nc = max(0, min(NHWC_TC, channels - c0));  // real channels in this chunk
-    const float* src = obs + ((size_t)b * channels + c0) * length;
     const int pitch = length + 1;
-    for (int i = threadIdx.x; i < nc * length; i += blockDim.x) {
-        const int c = i / length, l = i - c * length;
-        tile[c * pitch + l] = src[i];
+    if constexpr (kTwo) {
+        const int n1 = max(0, min(nc, c1 - c0));  // of which from obs
+        const float* src1 = obs + ((size_t)b * c1 + min(c0, c1)) * length;
+        const float* src2 = obs2 + ((size_t)b * c2 + max(0, c0 - c1)) * length;
+        for (int i = threadIdx.x; i < nc * length; i += blockDim.x) {
+            const int c = i / length, l = i - c * length;
+            tile[c * pitch + l] = c < n1 ? src1[i] : src2[i - n1 * length];
+        }
+    } else {
+        const float* src = obs + ((size_t)b * channels + c0) * length;
+        for (int i = threadIdx.x; i < nc * length; i += blockDim.x) {
+            const int c = i / length, l = i - c * length;
+            tile[c * pitch + l] = src[i];
+        }
     }
     __syncthreads();
     __nv_bfloat162* dst = reinterpret_cast<__nv_bfloat162*>(out + ((size_t)b * length) * cpad + c0);
@@ -219,6 +297,14 @@ __global__ void __launch_bounds__(256) k_obs_to_nhwc(const float* __restrict__ o
         const float a = c < nc ? tile[c * pitch + l] : 0.f, bb = c + 1 < nc ? tile[(c + 1) * pitch + l] : 0.f;
         dst[(size_t)l * (cpad / 2) + c / 2] = __floats2bfloat162_rn(a, bb);
     }
+}
+__global__ void __launch_bounds__(256) k_obs_to_nhwc(const float* __restrict__ obs, __nv_bfloat16* __restrict__ out, int channels, int length,
+                                                     int cpad) {
+    obs_chunk_to_nhwc<false>(obs, nullptr, out, channels, 0, length, cpad);
+}
+__global__ void __launch_bounds__(256) k_obs2_to_nhwc(const float* __restrict__ obs, const float* __restrict__ obs2,
+                                                      __nv_bfloat16* __restrict__ out, int c1, int c2, int length, int cpad) {
+    obs_chunk_to_nhwc<true>(obs, obs2, out, c1, c2, length, cpad);
 }
 
 }  // namespace mjx_nn

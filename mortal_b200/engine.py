@@ -19,7 +19,7 @@ class DeviceEngine:
 
     def __init__(self, brain, dqn, *, version=4, device=None, enable_amp=True, enable_quick_eval=True,
                  enable_rule_based_agari_guard=False, name="NoName", boltzmann_epsilon=0.0, boltzmann_temp=1.0,
-                 top_p=1.0, is_oracle=False, fast_inference=True):
+                 top_p=1.0, is_oracle=False, stochastic_latent=False, fast_inference=True):
         self.device = device or torch.device("cuda")
         self.brain = brain.to(self.device).eval()
         self.dqn = dqn.to(self.device).eval()
@@ -40,6 +40,7 @@ class DeviceEngine:
         self.boltzmann_epsilon = boltzmann_epsilon
         self.boltzmann_temp = boltzmann_temp
         self.top_p = top_p
+        self.stochastic_latent = stochastic_latent  # version 1: sample the latent from Normal(mu, exp(logsig) + 1e-6) instead of mu
         self._graphs = {}
 
     @torch.no_grad()
@@ -53,13 +54,15 @@ class DeviceEngine:
             self._graphs = {}
 
     @torch.inference_mode()
-    def react_device(self, obs: torch.Tensor, masks: torch.Tensor, return_greedy: bool = False):
-        """obs [B, C, 34] f32 cuda, masks [B, 46] bool cuda -> (actions int64 [B], q [B, 46][, is_greedy bool [B]])"""
+    def react_device(self, obs: torch.Tensor, masks: torch.Tensor, return_greedy: bool = False, invisible_obs=None):
+        """obs [B, C, 34] f32 cuda, masks [B, 46] bool cuda (invisible_obs [B, 211 | 217, 34] f32 cuda for oracle engines)
+        -> (actions int64 [B], q [B, 46][, is_greedy bool [B]])"""
+        inv = (invisible_obs,) if self.is_oracle else ()
         if self.fast:
-            q = self.dqn(self._fast_brain.forward_fast(obs).float(), masks)
+            q = self.dqn(self._latent(self._fast_brain.forward_fast(obs, *inv)).float(), masks)
         else:
             with torch.autocast(self.device.type, dtype=torch.bfloat16, enabled=self.enable_amp):
-                q = self.dqn(self.brain(obs), masks)
+                q = self.dqn(self._latent(self.brain(obs, *inv)), masks)
         if self.boltzmann_epsilon > 0:
             b = obs.shape[0]
             greedy = torch.full((b,), 1 - self.boltzmann_epsilon, device=self.device).bernoulli().to(torch.bool)
@@ -75,12 +78,22 @@ class DeviceEngine:
             return actions, q, greedy
         return actions, q
 
+    def _latent(self, out):
+        """version 1 brains return (mu, logsig) (mortal/engine.py:60-66): the DQN gets mu, or a sample with stochastic_latent"""
+        if not isinstance(out, tuple):
+            return out
+        mu, logsig = out
+        if self.stochastic_latent:
+            return torch.distributions.Normal(mu, logsig.exp() + 1e-6).sample()
+        return mu
+
     @torch.inference_mode()
     def react_static(self, obs_buf: torch.Tensor, masks_buf: torch.Tensor, nr: int, bucket: int = 256):
         """react_device(obs_buf[:nr], masks_buf[:nr]) for PERSISTENT buffers (BatchEnv.obs_buffer() / .masks): the forward
         over the first ceil(nr / bucket) * bucket rows is captured once per bucket as a CUDA graph and replayed, which
-        removes the ~600 kernel-launch calls per step from the host. Greedy engines only; rows past nr are stale and ignored."""
-        if self.boltzmann_epsilon > 0 or not self.fast:
+        removes the ~600 kernel-launch calls per step from the host. Greedy, non-oracle engines with a deterministic latent
+        only; rows past nr are stale and ignored."""
+        if self.boltzmann_epsilon > 0 or not self.fast or self.is_oracle or self.stochastic_latent:
             return self.react_device(obs_buf[:nr], masks_buf[:nr])
         nb = min(((nr + bucket - 1) // bucket) * bucket, obs_buf.shape[0])
         key = (obs_buf.data_ptr(), masks_buf.data_ptr(), nb)
@@ -105,7 +118,8 @@ class DeviceEngine:
     def react_batch(self, obs, masks, invisible_obs):
         o = torch.as_tensor(_stack_rows(obs), device=self.device)
         m = torch.as_tensor(_stack_rows(masks), device=self.device)
-        actions, q, greedy = self.react_device(o, m, return_greedy=True)
+        inv = None if invisible_obs is None else torch.as_tensor(_stack_rows(invisible_obs), device=self.device)
+        actions, q, greedy = self.react_device(o, m, return_greedy=True, invisible_obs=inv)
         return actions.tolist(), q.float().tolist(), m.tolist(), greedy.tolist()
 
 

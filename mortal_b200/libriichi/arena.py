@@ -162,10 +162,12 @@ class _Part:
         # agent/mortal.rs:253-255: engines with is_oracle also get the invisible observation (board.rs:680-782) of their rows
         self.oracle = [bool(getattr(a, "is_oracle", False)) for a in agents]
         self.version = version
-        self.h_inv = None
-        if any(self.oracle) and self.host_mode:
-            inv_rows = 211 if version == 1 else 217
-            self.h_inv = pin(torch.empty((env.row_cap, inv_rows, 34), dtype=torch.float32))
+        # each oracle engine gets the invisible observation in its own obs version (211 rows for version 1, 217 otherwise)
+        self.h_inv = [None, None]
+        if self.host_mode:
+            for k in range(2):
+                if self.oracle[k]:
+                    self.h_inv[k] = pin(torch.empty((env.row_cap, 211 if versions[k] == 1 else 217, 34), dtype=torch.float32))
         self.first, self.cycles, self.nr = True, 0, 0
         self.recorded, self.recorded_masks = [], []
         self.mask_weights = (1 << torch.arange(46, dtype=torch.int64))
@@ -245,13 +247,13 @@ class _Part:
                 same = agents[0] is agents[1]
                 groups = ((np.arange(nr), agents[0], self.oracle[0]),) if same else (
                     (np.nonzero(chal_h)[0], agents[0], self.oracle[0]), (np.nonzero(~chal_h)[0], agents[1], self.oracle[1]))
-                inv_np = None
-                if self.h_inv is not None:
-                    self.h_inv[:nr].copy_(env.encode_invisible(self.version)[:nr])
-                    inv_np = self.h_inv.numpy()
                 for k, (idx, agent, is_oracle) in enumerate(groups):
                     if idx.size == 0:
                         continue
+                    inv_np = None
+                    if is_oracle:
+                        self.h_inv[k][:nr].copy_(env.encode_invisible(self.versions[k])[:nr])
+                        inv_np = self.h_inv[k].numpy()
                     obs_np = self.obs_np
                     if self.mixed:  # each agent's rows in its own layout (mortal.rs:256-287): one encode per version
                         env.set_obs_version(self.versions[k])
@@ -259,7 +261,7 @@ class _Part:
                         assert env.encode_obs_host(buf, self.h_masks) == nr
                         obs_np = buf.numpy()
                     t_eval = time.perf_counter_ns()
-                    a, q, greedy = agent.react_host(obs_np, self.masks_np, idx, inv_np if is_oracle else None)
+                    a, q, greedy = agent.react_host(obs_np, self.masks_np, idx, inv_np)
                     if self.dev_meta:
                         ti = torch.from_numpy(idx)
                         self.h_mq[ti] = torch.from_numpy(q).reshape(-1, 46)
@@ -293,7 +295,6 @@ class _Part:
             obs, masks = obs_buf[:nr], env.masks[:nr]
             tbl = env.row_table[:nr].long()
             seat = (env.row_seat[:nr] & 3).long()
-            inv = env.encode_invisible(self.version)[:nr] if any(self.oracle) else None
             if agents[0] is agents[1]:  # one engine for every seat: no gather of the rows, CUDA-graph replay when the engine has one
                 agent = agents[0]
                 t_eval = time.perf_counter_ns()
@@ -301,7 +302,8 @@ class _Part:
                 if hasattr(agent, "react_static") and not meta_rec and not self.oracle[0]:
                     a, q = agent.react_static(obs_buf, env.masks, nr)
                 else:
-                    out = agent.react_device(obs, masks, invisible_obs=inv) if self.oracle[0] else agent.react_device(obs, masks)
+                    out = (agent.react_device(obs, masks, invisible_obs=env.encode_invisible(self.versions[0])[:nr]) if self.oracle[0]
+                           else agent.react_device(obs, masks))
                     a, q = out[0], out[1]
                 self.actions[:nr] = a.to(torch.int64)
                 if self.q_all is not None:
@@ -320,6 +322,7 @@ class _Part:
                         env.set_obs_version(self.versions[1])
                         obs = env.encode_obs()[:nr]
                         env.set_obs_version(self.versions[0])
+                    inv = env.encode_invisible(self.versions[k])[:nr] if is_oracle else None
                     t_eval = time.perf_counter_ns()
                     out = agent.react_device(obs[idx], masks[idx], invisible_obs=inv[idx]) if is_oracle else agent.react_device(obs[idx], masks[idx])
                     a, q = out[0], out[1]
