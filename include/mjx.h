@@ -360,6 +360,26 @@ int mjx_grp_reward_dev(int n_games, const double* feat, const int32_t* game_off,
                        const double* pts_host, int uniform_init, int64_t* steps_to_done, double* kyoku_reward,
                        int64_t* player_rank, int32_t* job_status, void* stream);
 
+/* ---- training-buffer observation records (csrc/mjx_obs_pack.cuh, layout: csrc/mjx_obs.cuh make_obs_record) ----------------
+ * A lossless fixed-size record per observation of (version 1..4, invisible 0 | 1): one uint64 column mask per row (bit c = the
+ * cell is 1.0; zero for a value row), then every value row verbatim as 34 floats, in ascending row order. Value rows: the
+ * encoder's (5 / 63 / 73 / 28 in versions 1..4) plus, in version 4, rows 889-890 and 961-1011 of the single-player block; the
+ * invisible observation's shanten / 6 rows in versions 2..4. Record bytes: 8,184 / 16,104 / 17,400 / 19,112 (versions 1..4),
+ * 1,688 / 2,144 (invisible, version 1 / 2..4); mjx_obs_record_bytes returns them (MJX_ERR_ARG for a bad version).
+ *   mjx_obs_pack_dev    obs float32 [n, rows, 34] with sample_pitch floats between samples (>= rows * 34; a slice of a larger
+ *                       tensor is read in place) -> records uint8 [n, record_bytes] (8-byte aligned) and status int32 [n]:
+ *                       0, or 1 + the first mask row holding a cell whose bits are neither +0.0 nor 1.0 (0.5, -0.0, NaN, 2.0 and
+ *                       denormals are refused, never rounded; the record is then not lossless). Value rows are copied bit for bit.
+ *   mjx_obs_unpack_dev  records [n_records, record_bytes], idx int64 [n_idx] (repeats allowed) -> out float32 [n_idx, rows, 34]
+ *                       (16-byte aligned), out[b] = the observation record idx[b] was packed from; an index outside
+ *                       [0, n_records) gives an all-zero observation.
+ * Device pointers; enqueued on `stream` without a synchronise. */
+int mjx_obs_record_bytes(int version, int invisible);
+int mjx_obs_pack_dev(int version, int invisible, long long n, const float* obs, long long sample_pitch, uint8_t* records,
+                     int32_t* status, void* stream);
+int mjx_obs_unpack_dev(int version, int invisible, const uint8_t* records, long long n_records, const int64_t* idx, long long n_idx,
+                       float* out, void* stream);
+
 /* ---- libriichi.state.PlayerState (state/player_state.rs:143-264, state/getter.rs:6-156, state/obs_repr.rs:776-791) ---------
  * A batch of n independent single-seat states: table records in single-seat mode (other seats' hidden tiles are `?` = 37), updated
  * by the same device event handlers self-play uses. `mjx_state_create` returns an mjx_env whose encoder entry points

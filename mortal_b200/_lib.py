@@ -127,6 +127,9 @@ SYMBOLS = {
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "mjx_grp_reward_dev": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_int, C.c_int,
                                      C.c_void_p, C.c_int, C.c_void_p, C.c_longlong] + [C.c_void_p] * 8 + [C.c_int] + [C.c_void_p] * 5),
+    "mjx_obs_record_bytes": (C.c_int, [C.c_int, C.c_int]),
+    "mjx_obs_pack_dev": (C.c_int, [C.c_int, C.c_int, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mjx_obs_unpack_dev": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p]),
 }
 
 

@@ -8,7 +8,11 @@
 
 namespace mjx {
 
-MJX_HD int oracle_obs_rows(int version) { return version == 1 ? 211 : 217; }
+MJX_HD constexpr int oracle_obs_rows(int version) { return version == 1 ? 211 : 217; }
+// the rows that hold a value other than 0 / 1: versions 2-4 write shanten / 6 into row 7 of each opponent's 8-row shanten block
+// (an opponent takes 4 + 3 + 8 + 1 + 1 = 17 rows); version 1 has none
+MJX_HD constexpr int oracle_obs_value_rows(int version) { return version == 1 ? 0 : 3; }
+MJX_HD constexpr int oracle_obs_value_row(int k) { return 17 * k + 4 + 3 + 7; }
 
 #ifdef MJX_HOST_EMUL
 #define INV_FOR(i, n) for (int i = 0; i < (n); i++)

@@ -18,6 +18,7 @@
 #include "mjx_grp.cuh"
 #include "mjx_reward.cuh"
 #include "mjx_invisible.cuh"
+#include "mjx_obs_pack.cuh"
 #include "mjx_state.cuh"
 #include "mjx_nn.cuh"
 #include "mjx_tables_host.h"
@@ -408,6 +409,60 @@ static_assert(ENCS_SMEM_BYTES <= 232448, "one CTA per SM");
 struct EncStoreArgs { int rows, bm_rows, n_sv, compact_bytes, n_slices, ver; };
 __constant__ short c_sv_row[4][OBS_MAX_SV];  // ObsLayout::sv_row of versions 1..4
 
+// One warp's items (row, slice) = item / n_slices, item % n_slices for item, item + stride, ... < n_items: materialise
+// the slice of output row `row` from the compact form at rec(row) (A.bm_rows masks, then A.n_sv value rows) into one of the
+// warp's two shared-memory tiles at `base` and store it to obs[row]. BULK: every slice starts and ends on a 16-byte boundary
+// (A.rows even) and leaves as a bulk asynchronous copy; otherwise the warp copies the tile out itself.
+template <bool BULK, typename Rec>
+__device__ __forceinline__ void enc_store_slices(const EncStoreArgs& A, Rec rec, const short* sv_row, int n_items, float* __restrict__ obs,
+                                                 unsigned char* base, int lane, int item, int stride, unsigned long long evict_first) {
+    u64 m0 = 0, m1 = 0;
+    if (item < n_items) {
+        const int row = item / A.n_slices;
+        enc_load_masks(reinterpret_cast<const u64*>(rec(row)), A.bm_rows, (item - row * A.n_slices) * OBS_SLICE_ROWS, lane, m0, m1);
+    }
+    for (int buf = 0; item < n_items; item += stride, buf ^= 1) {
+        const int row = item / A.n_slices, slice = item - row * A.n_slices;
+        const int row_lo = slice * OBS_SLICE_ROWS, row_hi = min(row_lo + OBS_SLICE_ROWS, A.rows);
+        // the next item's row masks are requested now and consumed one iteration later
+        u64 n0 = 0, n1 = 0;
+        if (item + stride < n_items) {
+            const int nrow = (item + stride) / A.n_slices;
+            enc_load_masks(reinterpret_cast<const u64*>(rec(nrow)), A.bm_rows, (item + stride - nrow * A.n_slices) * OBS_SLICE_ROWS,
+                           lane, n0, n1);
+        }
+        float* tile = reinterpret_cast<float*>(base + buf * ENC_SLICE_BYTES);
+        // the store that last used this tile (two items ago) must have finished reading it
+        if (BULK && lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
+        if (!BULK) {  // enc_materialize zeroes whole 16-byte words: clear the last two floats of a slice of an odd row count
+            const int n = (row_hi - row_lo) * OBS_COLS;
+            if ((n & ~3) + lane < n) tile[(n & ~3) + lane] = 0.f;
+        }
+        __syncwarp();
+        const unsigned char* cf = rec(row);
+        enc_materialize(reinterpret_cast<const float*>(cf + A.bm_rows * 8), sv_row, A.n_sv, lane, tile, row_lo, row_hi, m0, m1);
+        float* dst = obs + ((size_t)row * A.rows + row_lo) * OBS_COLS;
+        if (BULK) {
+            // make the generic-proxy smem writes visible to the async proxy, then one lane issues the bulk store
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            __syncwarp();
+            if (lane == 0) {
+                asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;"
+                             :: "l"(dst), "r"((unsigned)__cvta_generic_to_shared(tile)),
+                                "r"((unsigned)((row_hi - row_lo) * OBS_COLS * (int)sizeof(float))), "l"(evict_first)
+                             : "memory");
+                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+            }
+        } else {
+            __syncwarp();
+            for (int i = lane; i < (row_hi - row_lo) * OBS_COLS; i += 32) __stcs(dst + i, tile[i]);
+        }
+        m0 = n0; m1 = n1;
+    }
+    if (BULK && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+    __syncwarp();
+}
+
 __global__ void __launch_bounds__(ENCS_WARPS * 32, 1) k_encode_store(EnvView V, EncStoreArgs A, const unsigned char* __restrict__ compact,
                                                                      float* __restrict__ obs, int* __restrict__ work) {
     extern __shared__ __align__(128) unsigned char s_raw[];
@@ -421,44 +476,56 @@ __global__ void __launch_bounds__(ENCS_WARPS * 32, 1) k_encode_store(EnvView V, 
     // this kernel is reading (44 MB, written by k_encode_features just before)
     unsigned long long evict_first;
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(evict_first));
-    int item = blockIdx.x * ENCS_WARPS + warp;
-    u64 m0 = 0, m1 = 0;
-    if (item < n_items) {
-        const int row = item / A.n_slices;
-        enc_load_masks(reinterpret_cast<const u64*>(compact + (size_t)row * A.compact_bytes), A.bm_rows,
-                       (item - row * A.n_slices) * OBS_SLICE_ROWS, lane, m0, m1);
-    }
-    for (int buf = 0; item < n_items; item += stride, buf ^= 1) {
-        const int row = item / A.n_slices, slice = item - row * A.n_slices;
-        const int row_lo = slice * OBS_SLICE_ROWS, row_hi = min(row_lo + OBS_SLICE_ROWS, A.rows);
-        // the next item's row masks are requested now and consumed one iteration later
-        u64 n0 = 0, n1 = 0;
-        if (item + stride < n_items) {
-            const int nrow = (item + stride) / A.n_slices;
-            enc_load_masks(reinterpret_cast<const u64*>(compact + (size_t)nrow * A.compact_bytes), A.bm_rows,
-                           (item + stride - nrow * A.n_slices) * OBS_SLICE_ROWS, lane, n0, n1);
-        }
-        float* tile = reinterpret_cast<float*>(base + buf * ENC_SLICE_BYTES);
-        // the store that last used this tile (two items ago) must have finished reading it
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-        __syncwarp();
-        const unsigned char* cf = compact + (size_t)row * A.compact_bytes;
-        enc_materialize(reinterpret_cast<const float*>(cf + A.bm_rows * 8), sv_row, A.n_sv, lane, tile, row_lo, row_hi, m0, m1);
-        // make the generic-proxy smem writes visible to the async proxy, then one lane issues the bulk store
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) {
-            float* dst = obs + ((size_t)row * A.rows + row_lo) * OBS_COLS;
-            asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;"
-                         :: "l"(dst), "r"((unsigned)__cvta_generic_to_shared(tile)),
-                            "r"((unsigned)((row_hi - row_lo) * OBS_COLS * (int)sizeof(float))), "l"(evict_first)
-                         : "memory");
-            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-        m0 = n0; m1 = n1;
-    }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    __syncwarp();
+    enc_store_slices<true>(A, [&](int row) { return compact + (size_t)row * A.compact_bytes; }, sv_row, n_items, obs, base, lane,
+                           blockIdx.x * ENCS_WARPS + warp, stride, evict_first);
+}
+
+// ---- the training-buffer codec (csrc/mjx_obs_pack.cuh)
+__constant__ ObsRecord c_obs_rec[OBS_REC_KINDS] = {
+    make_obs_record(1, false), make_obs_record(2, false), make_obs_record(3, false), make_obs_record(4, false),
+    make_obs_record(1, true),  make_obs_record(2, true),  make_obs_record(3, true),  make_obs_record(4, true)};
+__constant__ ObsPackSlices c_pack_slices[OBS_REC_KINDS] = {
+    make_pack_slices(make_obs_record(1, false)), make_pack_slices(make_obs_record(2, false)),
+    make_pack_slices(make_obs_record(3, false)), make_pack_slices(make_obs_record(4, false)),
+    make_pack_slices(make_obs_record(1, true)),  make_pack_slices(make_obs_record(2, true)),
+    make_pack_slices(make_obs_record(3, true)),  make_pack_slices(make_obs_record(4, true))};
+// what an index outside [0, n_records) reads: an all-zero record (of the largest kind)
+__device__ u64 g_zero_record[(OBS_ROWS_V4 * 8 + OBS_REC_MAX_VAL * OBS_COLS * 4) / 8];
+
+// one CTA per sample, its warps over the 32-row slices; status = 1 + the first row with a cell other than +0.0 / 1.0, or 0
+__global__ void __launch_bounds__(OBS_PACK_WARPS * 32) k_obs_pack(int kind, const float* __restrict__ obs, long long pitch,
+                                                                  unsigned char* __restrict__ rec, int* __restrict__ status) {
+    __shared__ int s_bad;
+    const ObsRecord& R = c_obs_rec[kind];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const size_t i = blockIdx.x;
+    if (threadIdx.x == 0) s_bad = INT_MAX;
+    __syncthreads();
+    int bad = INT_MAX;
+    for (int lo = warp * OBS_PACK_SLICE; lo < R.rows; lo += OBS_PACK_WARPS * OBS_PACK_SLICE)
+        bad = min(bad, obs_pack_slice(R, c_pack_slices[kind], obs + i * pitch, rec + i * R.bytes, lo, lane));
+    if (lane == 0 && bad != INT_MAX) atomicMin(&s_bad, bad);
+    __syncthreads();
+    if (threadIdx.x == 0) status[i] = s_bad == INT_MAX ? 0 : s_bad + 1;
+}
+
+template <bool BULK>
+__global__ void __launch_bounds__(ENCS_WARPS * 32, 1) k_obs_unpack(int kind, const unsigned char* __restrict__ rec, long long n_rec,
+                                                                   const int64_t* __restrict__ idx, int n_idx, float* __restrict__ out) {
+    extern __shared__ __align__(128) unsigned char s_raw[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const ObsRecord& R = c_obs_rec[kind];
+    EncStoreArgs A;
+    A.rows = R.rows; A.bm_rows = R.rows; A.n_sv = R.n_val; A.compact_bytes = R.bytes;
+    A.n_slices = (R.rows + OBS_SLICE_ROWS - 1) / OBS_SLICE_ROWS; A.ver = kind % 4 + 1;
+    const auto record = [&](int b) {
+        const long long k = __ldg(idx + b);
+        return k >= 0 && k < n_rec ? rec + (size_t)k * R.bytes : reinterpret_cast<const unsigned char*>(g_zero_record);
+    };
+    unsigned long long evict_first;  // the batch streams through L2 without pushing out the records
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(evict_first));
+    enc_store_slices<BULK>(A, record, R.val_row, n_idx * A.n_slices, out, s_raw + (size_t)warp * 2 * ENC_SLICE_BYTES, lane,
+                           blockIdx.x * ENCS_WARPS + warp, gridDim.x * ENCS_WARPS, evict_first);
 }
 
 // invisible (oracle) observation of every row of the step: one warp per row (csrc/mjx_invisible.cuh)
@@ -1655,6 +1722,48 @@ int mjx_grp_reward_dev(int n_games, const double* feat, const int32_t* game_off,
     T.at_kyoku = at_kyoku; T.apply_gamma = apply_gamma; T.dones = dones;
     T.steps_to_done = steps_to_done; T.kyoku_reward = kyoku_reward; T.player_rank = player_rank; T.status = job_status;
     k_train_targets<<<(n_jobs + RW_WARPS - 1) / RW_WARPS, RW_WARPS * 32, 0, st>>>(T);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+// ---- training-buffer observation records (csrc/mjx_obs_pack.cuh)
+int mjx_obs_record_bytes(int version, int invisible) {
+    if (version < 1 || version > 4 || (invisible != 0 && invisible != 1))
+        return fail(MJX_ERR_ARG, "mjx_obs_record_bytes: version must be 1..4 and invisible 0 or 1");
+    return make_obs_record(version, invisible != 0).bytes;
+}
+
+int mjx_obs_pack_dev(int version, int invisible, long long n, const float* obs, long long sample_pitch, uint8_t* records,
+                     int32_t* status, void* stream) {
+    if (const char* why = obs_pack_check(version, invisible, n, obs, sample_pitch, records, status))
+        return fail(MJX_ERR_ARG, std::string("mjx_obs_pack_dev: ") + why);
+    if (n == 0) return MJX_OK;
+    k_obs_pack<<<(unsigned)n, OBS_PACK_WARPS * 32, 0, (cudaStream_t)stream>>>(obs_record_kind(version, invisible != 0), obs,
+                                                                                sample_pitch, records, status);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+int mjx_obs_unpack_dev(int version, int invisible, const uint8_t* records, long long n_records, const int64_t* idx, long long n_idx,
+                       float* out, void* stream) {
+    if (const char* why = obs_unpack_check(version, invisible, records, n_records, idx, n_idx, out))
+        return fail(MJX_ERR_ARG, std::string("mjx_obs_unpack_dev: ") + why);
+    if (n_idx == 0) return MJX_OK;
+    const int kind = obs_record_kind(version, invisible != 0);
+    const int rows = make_obs_record(version, invisible != 0).rows;
+    const long long items = n_idx * ((rows + OBS_SLICE_ROWS - 1) / OBS_SLICE_ROWS);
+    int dev = 0, sms = 0;
+    CU(cudaGetDevice(&dev));
+    CU(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const int grid = (int)std::min<long long>(sms, (items + ENCS_WARPS - 1) / ENCS_WARPS);  // one CTA per SM, as k_encode_store
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (rows % 2 == 0) {  // every slice 16-byte aligned: bulk stores
+        CU(cudaFuncSetAttribute(k_obs_unpack<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ENCS_SMEM_BYTES));
+        k_obs_unpack<true><<<grid, ENCS_WARPS * 32, ENCS_SMEM_BYTES, st>>>(kind, records, n_records, idx, (int)n_idx, out);
+    } else {
+        CU(cudaFuncSetAttribute(k_obs_unpack<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ENCS_SMEM_BYTES));
+        k_obs_unpack<false><<<grid, ENCS_WARPS * 32, ENCS_SMEM_BYTES, st>>>(kind, records, n_records, idx, (int)n_idx, out);
+    }
     CU(cudaGetLastError());
     return MJX_OK;
 }

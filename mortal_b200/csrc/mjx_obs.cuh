@@ -14,6 +14,7 @@
 // that leave the SM as bulk asynchronous copies (TMA, cp.async.bulk shared->global). Warps are independent
 // pipelines; there is no CTA-wide barrier anywhere.
 #pragma once
+#include "mjx_invisible.cuh"
 #include "mjx_step.cuh"
 
 namespace mjx {
@@ -127,6 +128,41 @@ static_assert(make_layout(1).rows == 938 && make_layout(2).rows == 942 && make_l
 static_assert(make_layout(3).n_sv <= OBS_MAX_SV && make_layout(2).n_sv <= OBS_MAX_SV, "value-row table size");
 // bytes of one compact observation: mask rows + value rows
 MJX_HD constexpr int enc_compact_bytes(int ver) { return make_layout(ver).bm_rows * 8 + make_layout(ver).n_sv * OBS_COLS * 4; }
+
+// The training-buffer record of one observation (k_obs_pack / k_obs_unpack, include/mjx.h mjx_obs_pack_dev): a 64-bit column
+// mask for EVERY row (zero for a value row), then the value rows verbatim, 34 floats each, in ascending row order. The value rows
+// are the encoder's sv_row plus, for version 4, the single-player block's non-0/1 rows (obs_repr.rs:563-690: 889-890, the two
+// rows of encode_ev, and 961-1011, encode_sp_table), so v4 has 28 + 53 = 81 of them, more than the encoder's own OBS_MAX_SV;
+// an invisible observation has oracle_obs_value_rows. Every other row holds only +0.0 and 1.0.
+constexpr int OBS_REC_MAX_VAL = 96;
+constexpr int OBS_REC_SP_EV = 2, OBS_REC_SP_TABLE0 = SP_ROW0 + 72;  // 889-890; 961-1011
+struct ObsRecord {
+    int rows, n_val, bytes;
+    short val_row[OBS_REC_MAX_VAL];
+};
+MJX_HD constexpr ObsRecord make_obs_record(int ver, bool invisible) {
+    ObsRecord R{};
+    int nv = 0;
+    if (invisible) {
+        R.rows = oracle_obs_rows(ver);
+        for (int k = 0; k < oracle_obs_value_rows(ver); k++) R.val_row[nv++] = (short)oracle_obs_value_row(k);
+    } else {
+        const ObsLayout L = make_layout(ver);
+        R.rows = L.rows;
+        for (int k = 0; k < L.n_sv; k++) R.val_row[nv++] = L.sv_row[k];
+        if (ver == 4) {
+            for (int r = SP_ROW0; r < SP_ROW0 + OBS_REC_SP_EV; r++) R.val_row[nv++] = (short)r;
+            for (int r = OBS_REC_SP_TABLE0; r < OBS_ROWS_V4; r++) R.val_row[nv++] = (short)r;
+        }
+    }
+    R.n_val = nv;
+    R.bytes = R.rows * 8 + nv * OBS_COLS * 4;
+    return R;
+}
+static_assert(make_obs_record(1, false).bytes == 8184 && make_obs_record(2, false).bytes == 16104 &&
+              make_obs_record(3, false).bytes == 17400 && make_obs_record(4, false).bytes == 19112 &&
+              make_obs_record(4, true).bytes == 2144 && make_obs_record(1, true).bytes == 1688, "record sizes");
+static_assert(make_obs_record(4, false).n_val == 81 && make_obs_record(4, false).n_val <= OBS_REC_MAX_VAL, "v4 value rows");
 
 struct EncCtx {
     const TableState* S;
@@ -519,14 +555,19 @@ MJX_DN void encode_obs_any(int ver, EncCtx& e, const Ctx& c, u64* mask_out) {
 // Called by ONE warp after encode_obs (and a warp sync). On the device the caller passes the slice's row masks
 // already in registers (lane l holds rows row_lo + l and row_lo + 32 + l), loaded ahead of time to hide their latency.
 #ifdef MJX_HOST_EMUL
-MJX_DN void enc_materialize(const ObsLayout& L, const EncCtx& e, float* tile, int row_lo, int row_hi) {
+// bm: bm_rows column masks; sv: n_sv value rows of 34 floats, row sv_row[k] each (a training-buffer record has the same form)
+MJX_DN void enc_materialize(const u64* bm, int bm_rows, const float* sv, const short* sv_row, int n_sv, float* tile, int row_lo,
+                            int row_hi) {
     for (int r = row_lo; r < row_hi; r++) {
-        const u64 m = r < L.bm_rows ? e.bm[r] : 0;
+        const u64 m = r < bm_rows ? bm[r] : 0;
         int slot = -1;
-        for (int k = 0; k < L.n_sv; k++) if (L.sv_row[k] == r) slot = k;
+        for (int k = 0; k < n_sv; k++) if (sv_row[k] == r) slot = k;
         for (int col = 0; col < 34; col++)
-            tile[(r - row_lo) * 34 + col] = slot >= 0 ? e.sv[slot * 34 + col] : (((m >> col) & 1) ? 1.f : 0.f);
+            tile[(r - row_lo) * 34 + col] = slot >= 0 ? sv[slot * 34 + col] : (((m >> col) & 1) ? 1.f : 0.f);
     }
+}
+MJX_DN void enc_materialize(const ObsLayout& L, const EncCtx& e, float* tile, int row_lo, int row_hi) {
+    enc_materialize(e.bm, L.bm_rows, e.sv, L.sv_row, L.n_sv, tile, row_lo, row_hi);
 }
 #else
 static_assert(OBS_SLICE_ROWS <= 64, "two mask words per lane cover a slice");

@@ -172,19 +172,12 @@ class RewardCalculator:
         return delta_points
 
 
-def training_samples(data, reward_calc: RewardCalculator):
-    """dataloader.py populate_buffer over a whole GameplayLoader result (list per file of list of Gameplay): the buffer's entries
-    before its shuffle (file, then Gameplay, then move) as device tensors on reward_calc.device, a dict of
-        obs            float32 [N, C, 34]
-        invisible_obs  float32 [N, C', 34], only when the loader had oracle=True (and some Gameplay has moves)
-        actions        int64 [N]
-        masks          bool [N, 46]
-        steps_to_done  int64 [N]
-        kyoku_rewards  float64 [N]
-        player_ranks   int64 [N]
-    The GRP runs once per game (a log's Gameplays share its Grp). Raises the reference's AssertionError where a Gameplay's
-    at_kyoku[-1] + 1 exceeds its game's kyoku count. A Gameplay with no moves contributes no samples (the reference fails on
-    it with an IndexError)."""
+def gameplay_targets(data, reward_calc: RewardCalculator):
+    """the per-move targets of dataloader.py populate_buffer over a whole GameplayLoader result, in buffer order (file, then
+    Gameplay, then move) -> (the Gameplays with moves, dict of device tensors on reward_calc.device: actions int64 [N], masks bool
+    [N, 46], steps_to_done int64 [N], kyoku_rewards float64 [N], player_ranks int64 [N]). The GRP runs once per game (a log's
+    Gameplays share its Grp). Raises the reference's AssertionError where a Gameplay's at_kyoku[-1] + 1 exceeds its game's kyoku
+    count."""
     dev = reward_calc.device
     gps = [gp for file in data for gp in file]
     games, slot, feats = [], {}, []
@@ -201,17 +194,11 @@ def training_samples(data, reward_calc: RewardCalculator):
             feats.append(_feature(grp.take_feature()))
         assert len(feats[g]) >= int(at_kyoku[-1]) + 1  # usually they are equal, unless there is no action in the last kyoku
         jobs.append(gp); job_game.append(g); job_player.append(gp.take_player_id()); counts.append(len(at_kyoku))
-    oracle = bool(jobs) and all(gp._invisible is not None for gp in jobs)
     with torch.cuda.device(dev):
-        cat = lambda xs, empty: torch.cat([x.to(dev) for x in xs]) if xs else empty
-        out = dict(obs=cat([gp.take_obs() for gp in jobs], torch.zeros((0, 0, 34), device=dev)))
-        if oracle:
-            out["invisible_obs"] = cat([gp.take_invisible_obs() for gp in jobs], torch.zeros((0, 0, 34), device=dev))
         if not jobs:
             z = torch.zeros(0, dtype=torch.int64, device=dev)
-            out.update(actions=z, masks=torch.zeros((0, 46), dtype=torch.bool, device=dev), steps_to_done=z.clone(),
-                       kyoku_rewards=torch.zeros(0, dtype=torch.float64, device=dev), player_ranks=z.clone())
-            return out
+            return jobs, dict(actions=z, masks=torch.zeros((0, 46), dtype=torch.bool, device=dev), steps_to_done=z.clone(),
+                              kyoku_rewards=torch.zeros(0, dtype=torch.float64, device=dev), player_ranks=z.clone())
         move_off = np.zeros(len(jobs) + 1, dtype=np.int32)
         np.cumsum(counts, out=move_off[1:])
         host = dict(move_off=move_off, job_game=np.array(job_game, dtype=np.int32), job_player=np.array(job_player, dtype=np.uint8),
@@ -221,9 +208,33 @@ def training_samples(data, reward_calc: RewardCalculator):
                     rank=np.array([g.take_rank_by_player() for g in games], dtype=np.uint8),
                     final=np.array([g.take_final_scores() for g in games], dtype=np.int64))
         _, (steps, reward, rank, status) = reward_calc._launch(feats, host)
-        out["actions"] = torch.from_numpy(np.concatenate([np.asarray(gp._actions, dtype=np.int64) for gp in jobs])).to(dev)
-        out["masks"] = cat([gp.take_masks() for gp in jobs], None)
-        out.update(steps_to_done=steps, kyoku_rewards=reward, player_ranks=rank)
+        out = dict(actions=torch.from_numpy(np.concatenate([np.asarray(gp._actions, dtype=np.int64) for gp in jobs])).to(dev),
+                   masks=torch.cat([gp.take_masks().to(dev) for gp in jobs]), steps_to_done=steps, kyoku_rewards=reward,
+                   player_ranks=rank)
         if (status != 0).any():
             raise RuntimeError(f"mjx_grp_reward_dev: job statuses {status.cpu().numpy().tolist()}")
+    return jobs, out
+
+
+def training_samples(data, reward_calc: RewardCalculator):
+    """dataloader.py populate_buffer over a whole GameplayLoader result (list per file of list of Gameplay): the buffer's entries
+    before its shuffle (file, then Gameplay, then move) as device tensors on reward_calc.device, a dict of
+        obs            float32 [N, C, 34]
+        invisible_obs  float32 [N, C', 34], only when the loader had oracle=True (and some Gameplay has moves)
+        actions        int64 [N]
+        masks          bool [N, 46]
+        steps_to_done  int64 [N]
+        kyoku_rewards  float64 [N]
+        player_ranks   int64 [N]
+    with the targets of gameplay_targets. A Gameplay with no moves contributes no samples (the reference fails on it with an
+    IndexError)."""
+    dev = reward_calc.device
+    jobs, targets = gameplay_targets(data, reward_calc)
+    oracle = bool(jobs) and all(gp._invisible is not None for gp in jobs)
+    with torch.cuda.device(dev):
+        cat = lambda xs: torch.cat([x.to(dev) for x in xs]) if xs else torch.zeros((0, 0, 34), device=dev)
+        out = dict(obs=cat([gp.take_obs() for gp in jobs]))
+        if oracle:
+            out["invisible_obs"] = cat([gp.take_invisible_obs() for gp in jobs])
+    out.update(targets)
     return out
