@@ -360,6 +360,38 @@ int mjx_grp_reward_dev(int n_games, const double* feat, const int32_t* game_off,
                        const double* pts_host, int uniform_init, int64_t* steps_to_done, double* kyoku_reward,
                        int64_t* player_rank, int32_t* job_status, void* stream);
 
+/* ---- GRP training step: mortal/train_grp.py:45-81, 172-186 over model.py:233-286 (csrc/mjx_grp_train.cuh) -------------------
+ * The per-sample status: OK; GAME: the sample's job is out of range, its game is not the job's, or the job's game, offsets or step
+ * count are out of range; LEN: the prefix length is outside 1..the job's steps. A sample that is not OK contributes nothing. */
+enum mjx_grp_train_status { MJX_GRP_TRAIN_OK = 0, MJX_GRP_TRAIN_GAME = 1, MJX_GRP_TRAIN_LEN = 2 };
+/* One training step of the GRP (the reference's populate_buffer prefixes, collate's pack_padded_sequence, forward_packed,
+ * get_label, F.cross_entropy, loss.backward()) over B = n_samples samples, each the prefix feature[:len] of one game with that
+ * game's rank_by_player. Device pointers unless stated; float64 throughout.
+ *   feat, game_off, n_rows, n_games   the games' kyoku rows, as mjx_grp_reward_dev takes them (n_rows >= 1);
+ *   weights, n_weights, hidden, layers  the packed net, as mjx_grp_reward_dev takes it;
+ *   sample_game int32 [B], sample_len int32 [B], rank_by_player int64 [B, 4]: the samples (populate_buffer's (feature[:len],
+ *                rank_by_player)); a rank row that is no permutation of 0..3 gets label 0, as get_label leaves it;
+ *   jobs         the samples grouped by game: job j steps game job_game[j] (int32 [n_jobs]) for job_steps[j] (int32) steps, the
+ *                longest prefix of its samples, at most max_steps (host int); sample b belongs to job sample_job[b] (int32 [B]);
+ *                the samples of job j are job_sample[job_sample_off[j] .. job_sample_off[j + 1]) (int32 [n_jobs + 1], [B]).
+ *                A (game, len) pair may appear more than once; each appearance counts.
+ *   loss, acc    out float64 scalars: F.cross_entropy(logits, labels) (the mean over B) and (argmax == label).mean(), argmax
+ *                taking the first maximum;
+ *   grad         out float64 [n_weights] in the weights' layout: d loss / d weights, as loss.backward() leaves them; null =
+ *                forward only (nothing written there);
+ *   sample_status out int32 [B] mjx_grp_train_status;
+ *   scratch      at least mjx_grp_train_scratch_bytes(hidden, layers, B, n_jobs, max_steps) bytes, 8-byte aligned.
+ * MJX_ERR_ARG for a bad count, shape, weight count, null pointer or short scratch. Enqueued on `stream` without a synchronise;
+ * every index read is checked against n_games, n_rows, n_jobs and B. Deterministic: no atomics, fixed reduction orders. */
+int mjx_grp_train_dev(int n_games, const double* feat, const int32_t* game_off, long long n_rows, const double* weights,
+                      long long n_weights, int hidden, int layers, int n_samples, const int32_t* sample_game, const int32_t* sample_len,
+                      const int64_t* rank_by_player, int n_jobs, const int32_t* job_game, const int32_t* job_steps,
+                      const int32_t* sample_job, const int32_t* job_sample_off, const int32_t* job_sample, int max_steps, double* loss,
+                      double* acc, double* grad, int32_t* sample_status, void* scratch, long long scratch_bytes, void* stream);
+/* the scratch bytes of mjx_grp_train_dev; MJX_ERR_ARG unless 1 <= hidden <= 256, 1 <= layers <= 4, 1 <= n_samples <= 2^24,
+ * 1 <= n_jobs <= n_samples, 1 <= max_steps <= 65536 */
+long long mjx_grp_train_scratch_bytes(int hidden, int layers, int n_samples, int n_jobs, int max_steps);
+
 /* ---- training-buffer observation records (csrc/mjx_obs_pack.cuh, layout: csrc/mjx_obs.cuh make_obs_record) ----------------
  * A lossless fixed-size record per observation of (version 1..4, invisible 0 | 1): one uint64 column mask per row (bit c = the
  * cell is 1.0; zero for a value row), then every value row verbatim as 34 floats, in ascending row order. Value rows: the

@@ -127,6 +127,10 @@ SYMBOLS = {
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "mjx_grp_reward_dev": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_int, C.c_int,
                                      C.c_void_p, C.c_int, C.c_void_p, C.c_longlong] + [C.c_void_p] * 8 + [C.c_int] + [C.c_void_p] * 5),
+    "mjx_grp_train_dev": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_int, C.c_int,
+                                    C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 5
+                                   + [C.c_int] + [C.c_void_p] * 5 + [C.c_longlong, C.c_void_p]),
+    "mjx_grp_train_scratch_bytes": (C.c_longlong, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "mjx_obs_record_bytes": (C.c_int, [C.c_int, C.c_int]),
     "mjx_obs_pack_dev": (C.c_int, [C.c_int, C.c_int, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p]),
     "mjx_obs_unpack_dev": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p]),

@@ -17,6 +17,7 @@
 #include "mjx_stat.cuh"
 #include "mjx_grp.cuh"
 #include "mjx_reward.cuh"
+#include "mjx_grp_train.cuh"
 #include "mjx_invisible.cuh"
 #include "mjx_obs_pack.cuh"
 #include "mjx_state.cuh"
@@ -1722,6 +1723,50 @@ int mjx_grp_reward_dev(int n_games, const double* feat, const int32_t* game_off,
     T.at_kyoku = at_kyoku; T.apply_gamma = apply_gamma; T.dones = dones;
     T.steps_to_done = steps_to_done; T.kyoku_reward = kyoku_reward; T.player_rank = player_rank; T.status = job_status;
     k_train_targets<<<(n_jobs + RW_WARPS - 1) / RW_WARPS, RW_WARPS * 32, 0, st>>>(T);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+// ---- GRP training step (train_grp.py:45-81, 172-186; model.py:233-286)
+long long mjx_grp_train_scratch_bytes(int hidden, int layers, int n_samples, int n_jobs, int max_steps) {
+    const long long b = rt_scratch_bytes(hidden, layers, n_samples, n_jobs, max_steps);
+    return b < 0 ? fail(MJX_ERR_ARG, "mjx_grp_train_scratch_bytes: bad counts") : b;
+}
+
+int mjx_grp_train_dev(int n_games, const double* feat, const int32_t* game_off, long long n_rows, const double* weights,
+                      long long n_weights, int hidden, int layers, int n_samples, const int32_t* sample_game, const int32_t* sample_len,
+                      const int64_t* rank_by_player, int n_jobs, const int32_t* job_game, const int32_t* job_steps,
+                      const int32_t* sample_job, const int32_t* job_sample_off, const int32_t* job_sample, int max_steps, double* loss,
+                      double* acc, double* grad, int32_t* sample_status, void* scratch, long long scratch_bytes, void* stream) {
+    if (rt_check_args(n_games, feat, game_off, n_rows, weights, n_weights, hidden, layers, n_samples, sample_game, sample_len,
+                      rank_by_player, n_jobs, job_game, job_steps, sample_job, job_sample_off, job_sample, max_steps, loss, acc,
+                      sample_status, scratch, scratch_bytes) ||
+        ((uintptr_t)scratch & 7))
+        return fail(MJX_ERR_ARG, "mjx_grp_train_dev: bad arguments");
+    const cudaStream_t st = (cudaStream_t)stream;
+    TrainView V{};
+    V.feat = feat; V.game_off = game_off; V.n_rows = n_rows; V.n_games = n_games; V.net = GrpNet{weights, hidden, layers};
+    V.n_samples = n_samples; V.sample_game = sample_game; V.sample_len = sample_len; V.rank = rank_by_player;
+    V.n_jobs = n_jobs; V.max_steps = max_steps; V.job_game = job_game; V.job_steps = job_steps; V.sample_job = sample_job;
+    V.job_sample_off = job_sample_off; V.job_sample = job_sample; V.loss = loss; V.acc = acc; V.grad = grad; V.status = sample_status;
+    V = rt_view(V, (double*)scratch);
+    const int smem_f = rw_smem_doubles(hidden, layers) * (int)sizeof(double);
+    const int smem_h = rt_head_smem_doubles(hidden, layers) * (int)sizeof(double);
+    const int smem_b = rt_bwd_smem_doubles(hidden, layers) * (int)sizeof(double);
+    if (smem_f > 48 * 1024) CU(cudaFuncSetAttribute(k_grp_train_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_f));
+    if (smem_h > 48 * 1024) CU(cudaFuncSetAttribute(k_grp_train_head, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_h));
+    k_grp_train_fwd<<<(n_jobs + RW_GAMES - 1) / RW_GAMES, RT_THREADS, smem_f, st>>>(V);
+    CU(cudaGetLastError());
+    k_grp_train_head<<<(n_samples + RW_GAMES - 1) / RW_GAMES, RT_THREADS, smem_h, st>>>(V);
+    CU(cudaGetLastError());
+    if (grad) {
+        k_grp_train_bwd<<<n_jobs, RT_THREADS, smem_b, st>>>(V);
+        CU(cudaGetLastError());
+        const RtWgrad W = rt_wgrad_segs(V);
+        k_grp_train_wgrad<<<W.n_tiles, RT_THREADS, 0, st>>>(W);
+        CU(cudaGetLastError());
+    }
+    k_grp_train_loss<<<1, RT_THREADS, 0, st>>>(V);
     CU(cudaGetLastError());
     return MJX_OK;
 }

@@ -168,9 +168,25 @@ MJX_D void rw_load_x(const MatrixView& V, const RwCta& C, int t, int tid) {
     }
 }
 
-// layer k of the GRU, the new hidden state of unit j for every game (torch's cell: r = σ(W_ir x + b_ir + W_hr h + b_hr),
-// z likewise, n = tanh(W_in x + b_in + r ⊙ (W_hn h + b_hn)), h' = (1 − z) ⊙ n + z ⊙ h); returns the unit this thread writes, or -1
-MJX_D int rw_gru_compute(const GrpNet& n, const RwCta& C, int k, int tid, double (&hn)[RW_GAMES]) {
+// torch's GRU cell gates of unit j from the input (gi) and hidden (gh) dot products of its three gate rows (r, z, n):
+// r = σ(W_ir x + b_ir + W_hr h + b_hr), z likewise, hn = W_hn h + b_hn, n = tanh(W_in x + b_in + r ⊙ hn)
+struct RwGates {
+    double r, z, n, hn;
+};
+
+MJX_D RwGates rw_gru_gates(const double* bih, const double* bhh, int H, int j, double gir, double giz, double gin, double ghr,
+                           double ghz, double ghn) {
+    RwGates G;
+    G.r = rw_sigmoid(gir + MJX_LDG(bih + j) + ghr + MJX_LDG(bhh + j));
+    G.z = rw_sigmoid(giz + MJX_LDG(bih + H + j) + ghz + MJX_LDG(bhh + H + j));
+    G.hn = ghn + MJX_LDG(bhh + 2 * H + j);
+    G.n = tanh(gin + MJX_LDG(bih + 2 * H + j) + G.r * G.hn);
+    return G;
+}
+
+// layer k of the GRU, the new hidden state of unit j for every game (rw_gru_gates, h' = (1 − z) ⊙ n + z ⊙ h); returns the unit
+// this thread writes, or -1. `gates` (optional) receives every game's gates of that unit.
+MJX_D int rw_gru_compute(const GrpNet& n, const RwCta& C, int k, int tid, double (&hn)[RW_GAMES], RwGates* gates = nullptr) {
     const int H = n.H, hl = H * n.layers, in = n.in(k), ks = rw_slices(H), j = tid / ks, s = tid % ks;
     const double* wih = n.layer(k);
     const double* whh = wih + 3LL * H * in;
@@ -196,10 +212,10 @@ MJX_D int rw_gru_compute(const GrpNet& n, const RwCta& C, int k, int tid, double
     rw_reduce(gh, ks);
     if (j >= H || s) return -1;
     for (int g = 0; g < RW_GAMES; g++) {
-        const double r = rw_sigmoid(gi[g] + MJX_LDG(bih + j) + gh[g] + MJX_LDG(bhh + j));
-        const double z = rw_sigmoid(gi[RW_GAMES + g] + MJX_LDG(bih + H + j) + gh[RW_GAMES + g] + MJX_LDG(bhh + H + j));
-        const double nn = tanh(gi[2 * RW_GAMES + g] + MJX_LDG(bih + 2 * H + j) + r * (gh[2 * RW_GAMES + g] + MJX_LDG(bhh + 2 * H + j)));
-        hn[g] = (1.0 - z) * nn + z * h[g * hl + j];
+        const RwGates G = rw_gru_gates(bih, bhh, H, j, gi[g], gi[RW_GAMES + g], gi[2 * RW_GAMES + g], gh[g], gh[RW_GAMES + g],
+                                       gh[2 * RW_GAMES + g]);
+        hn[g] = (1.0 - G.z) * G.n + G.z * h[g * hl + j];
+        if (gates) gates[g] = G;
     }
     return j;
 }

@@ -13,6 +13,7 @@ The modules use their own parameter names; `load_mortal` is the one place that k
 """
 from __future__ import annotations
 
+import itertools
 import re
 
 import torch
@@ -270,6 +271,29 @@ class DQN(nn.Module):
             v, a = self.v_head(phi), self.a_head(phi)
         a_mean = a.masked_fill(~mask, 0.0).sum(-1, keepdim=True) / mask.sum(-1, keepdim=True)
         return (v + a - a_mean).masked_fill(~mask, -torch.inf)
+
+
+class GRP(nn.Module):
+    """mortal/model.py:233-286 GRP's parameters and buffers: GRU(7 -> hidden_size, num_layers), fc = Linear(HL, HL), ReLU,
+    Linear(HL, 24), HL = hidden_size * num_layers, float64, and the `perms` (24, 4) / `perms_t` (4, 24) buffers of
+    itertools.permutations(range(4)). Its state dict has the reference's keys, order, shapes and dtypes, so a reference `grp.pth`
+    loads strictly here and back, and the parameters are created in the reference's order (the same torch seed gives the same
+    initial weights). There is no torch forward: the net runs as device kernels, `grp_train.grp_loss` for training and
+    `reward.RewardCalculator` for the rank probabilities."""
+
+    def __init__(self, hidden_size=64, num_layers=2):
+        super().__init__()
+        self.rnn = nn.GRU(input_size=7, hidden_size=hidden_size, num_layers=num_layers, batch_first=True)
+        hl = hidden_size * num_layers
+        self.fc = nn.Sequential(nn.Linear(hl, hl), nn.ReLU(inplace=True), nn.Linear(hl, 24))
+        for mod in self.modules():
+            mod.to(torch.float64)
+        perms = torch.tensor(list(itertools.permutations(range(4))))
+        self.register_buffer("perms", perms)
+        self.register_buffer("perms_t", perms.transpose(0, 1))
+
+    def forward(self, *args, **kwargs):
+        raise NotImplementedError("GRP has no torch forward: use mortal_b200.grp_train.grp_loss or mortal_b200.reward.RewardCalculator")
 
 
 # ---- Mortal checkpoints ------------------------------------------------------------------------------------------------------
