@@ -522,6 +522,50 @@ int mjx_nn_post_block_tail_bf16(const void* y, const void* x, const float* scale
 int mjx_nn_obs2_to_nhwc_bf16(const float* obs, const float* obs2, void* out, int batch, int channels, int channels2, int length,
                              int channels_padded, void* stream);
 
+/* ---- policy-net training (mortal/train.py:228-248; csrc/mjx_train.cuh) ------------------------------------------------------
+ * Activations are channels-last [batch, length, channels] (rows = batch * length), stored as `dtype` MJX_TRAIN_F32 or
+ * MJX_TRAIN_F16, fp32 arithmetic; 1 <= channels <= 256 with channels % 8 == 0, batch >= 1. Per-channel vectors (gamma, beta,
+ * running stats, mean / invstd, dgamma / dbeta) are float32. Reductions run in an order fixed by the shape: equal inputs give
+ * bit-identical outputs. Non-finite values pass through unclamped. MJX_ERR_ARG for a bad dtype, shape or null pointer. */
+enum mjx_train_dtype { MJX_TRAIN_F32 = 0, MJX_TRAIN_F16 = 1 };
+/* float32 elements of the scratch the two BatchNorm calls need for `rows` x `channels` */
+long long mjx_train_bn_scratch_floats(int rows, int channels);
+/* out = mish(gamma (x - mean) invstd + beta). training != 0: mean / biased variance of the batch (per-block shifted sums merged
+ * as (count, mean, M2) in double), running_mean / running_var updated with `momentum` (running_var from the unbiased variance),
+ * save_mean / save_invstd written; training == 0: the running statistics are used and left untouched (save_* still written).
+ * save_mean is float32 [2 * channels], the mean as a pair hi [0, channels) + lo [channels, 2 * channels); save_invstd
+ * float32 [channels]. */
+int mjx_train_bn_mish_fwd(int dtype, const void* x, const float* gamma, const float* beta, float* running_mean, float* running_var,
+                          float* save_mean, float* save_invstd, void* out, int rows, int channels, float eps, float momentum,
+                          int training, float* scratch, void* stream);
+/* the backward of mjx_train_bn_mish_fwd from its x, save_mean and save_invstd: dx, dgamma = sum dz xhat, dbeta = sum dz,
+ * dz = dout mish'(u); training == 0 gives the backward of the affine map (frozen BatchNorm). */
+int mjx_train_bn_mish_bwd(int dtype, const void* x, const void* dout, const float* gamma, const float* beta, const float* save_mean,
+                          const float* save_invstd, void* dx, float* dgamma, float* dbeta, int rows, int channels, int training,
+                          float* scratch, void* stream);
+/* the channel gate: avg / mx [batch, channels] = mean / max over length of y */
+int mjx_train_gate_pool(int dtype, const void* y, void* avg, void* mx, int batch, int length, int channels, void* stream);
+/* out = y * g[b, c] + x, g [batch, channels] */
+int mjx_train_gate_out(int dtype, const void* y, const void* g, const void* x, void* out, int batch, int length, int channels,
+                       void* stream);
+/* dg float32 [batch, channels] = sum_l dout y; cnt float32 [batch, channels] = the number of l with y == mx */
+int mjx_train_gate_bwd_dg(int dtype, const void* dout, const void* y, const void* mx, float* dg, float* cnt, int batch, int length,
+                          int channels, void* stream);
+/* dy = dout g + davg / length + (y == mx ? dmx / cnt : 0) */
+int mjx_train_gate_bwd_dy(int dtype, const void* dout, const void* y, const void* g, const void* mx, const float* cnt,
+                          const void* davg, const void* dmx, void* dy, int batch, int length, int channels, void* stream);
+/* The dueling combine and the three losses of one batch in one launch. v [batch], a [batch, 46], aux [batch, n_aux] (dtype),
+ * masks uint8 [batch, 46], actions / steps_to_done / ranks int64 [batch], rewards float64 [batch]. Writes q_out float32
+ * [batch, 46] (optional: NULL skips it), q_act / q_target float32 [batch], losses float32 [3] = (0.5 mse, mean lse - mean q,
+ * cross-entropy), and ORs 1 into *bad when an action is outside its mask. 1 <= n_aux <= 32. */
+int mjx_train_dqn_loss_fwd(int dtype, const void* v, const void* a, const uint8_t* masks, const int64_t* actions,
+                           const int64_t* steps_to_done, const double* rewards, const void* aux, const int64_t* ranks, int batch,
+                           int n_aux, float gamma, float* q_out, float* q_act, float* q_target, float* losses, int* bad, void* stream);
+/* gradients of w[0] dqn + w[1] cql + w[2] next_rank (w float32 [3], device) for v, a and aux, from q_target of the forward */
+int mjx_train_dqn_loss_bwd(int dtype, const void* v, const void* a, const uint8_t* masks, const int64_t* actions,
+                           const float* q_target, const void* aux, const int64_t* ranks, int batch, int n_aux, const float* w,
+                           void* dv, void* da, void* daux, void* stream);
+
 /* ---- standalone kernels (BASELINE configs 3/4) ------------------------------------------------ */
 /* algo/shanten.rs:138-150 calc_all: tiles_dev uint8 [n,34], len_div3_dev uint8 [n] -> int8 [n]. */
 int mjx_shanten(const uint8_t* tiles_dev, const uint8_t* len_div3_dev, int8_t* out_dev, int n, void* stream);

@@ -81,6 +81,16 @@ SYMBOLS = {
     "mjx_nn_affine_relu_bf16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_void_p]),
     "mjx_nn_post_block_tail_bf16": (C.c_int, [C.c_void_p] * 10 + [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "mjx_nn_obs2_to_nhwc_bf16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int] * 5 + [C.c_void_p]),
+    "mjx_train_bn_scratch_floats": (C.c_longlong, [C.c_int, C.c_int]),
+    "mjx_train_bn_mish_fwd": (C.c_int, [C.c_int] + [C.c_void_p] * 8 + [C.c_int, C.c_int, C.c_float, C.c_float, C.c_int, C.c_void_p,
+                                                                         C.c_void_p]),
+    "mjx_train_bn_mish_bwd": (C.c_int, [C.c_int] + [C.c_void_p] * 9 + [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "mjx_train_gate_pool": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "mjx_train_gate_out": (C.c_int, [C.c_int] + [C.c_void_p] * 4 + [C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "mjx_train_gate_bwd_dg": (C.c_int, [C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "mjx_train_gate_bwd_dy": (C.c_int, [C.c_int] + [C.c_void_p] * 8 + [C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "mjx_train_dqn_loss_fwd": (C.c_int, [C.c_int] + [C.c_void_p] * 8 + [C.c_int, C.c_int, C.c_float] + [C.c_void_p] * 6),
+    "mjx_train_dqn_loss_bwd": (C.c_int, [C.c_int] + [C.c_void_p] * 7 + [C.c_int, C.c_int] + [C.c_void_p] * 5),
     "mjx_env_create_replay": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p,
                                         C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_int]),
     "mjx_env_create_replay_dev": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong,

@@ -22,6 +22,7 @@
 #include "mjx_obs_pack.cuh"
 #include "mjx_state.cuh"
 #include "mjx_nn.cuh"
+#include "mjx_train.cuh"
 #include "mjx_tables_host.h"
 
 using namespace mjx;
@@ -2294,6 +2295,135 @@ int mjx_make_wall_host(uint64_t nonce, uint64_t key, int kyoku, int honba, int s
     CU(cudaGetLastError());
     CU(cudaMemcpy(wall136, d, 136, cudaMemcpyDeviceToHost));
     cudaFree(d);
+    return MJX_OK;
+}
+
+// ---- policy-net training (csrc/mjx_train.cuh) ---------------------------------------------------------------------------------
+// grids depend on the shape only (not on the device), so the reduction order, and with it every bit of the result, does too
+static int train_grid(size_t n) { const size_t g = (n + 255) / 256; return (int)(g < 4096 ? (g ? g : 1) : 4096); }
+static bool train_shape_ok(int dtype, int rows, int channels, int length = 1) {  // elementwise passes index in 32 bits
+    return (dtype == MJX_TRAIN_F32 || dtype == MJX_TRAIN_F16) && rows > 0 && channels > 0 && channels <= 256 && channels % 8 == 0 &&
+           length > 0 && (long long)rows * length * channels < (1LL << 31);
+}
+#define MJX_TRAIN_DISPATCH(dtype, ...)                       \
+    do {                                                     \
+        if ((dtype) == MJX_TRAIN_F32) {                      \
+            using T = float;                                 \
+            __VA_ARGS__;                                     \
+        } else {                                             \
+            using T = __half;                                \
+            __VA_ARGS__;                                     \
+        }                                                    \
+    } while (0)
+
+long long mjx_train_bn_scratch_floats(int rows, int channels) {
+    if (rows <= 0 || channels <= 0) return 0;
+    return 4LL * mjx_train::bn_blocks(rows) * channels + 3LL * channels;
+}
+int mjx_train_bn_mish_fwd(int dtype, const void* x, const float* gamma, const float* beta, float* running_mean, float* running_var,
+                          float* save_mean, float* save_invstd, void* out, int rows, int channels, float eps, float momentum,
+                          int training, float* scratch, void* stream) {
+    if (!train_shape_ok(dtype, rows, channels) || !x || !gamma || !beta || !running_mean || !running_var || !save_mean ||
+        !save_invstd || !out || !scratch || (training && rows < 2))
+        return fail(MJX_ERR_ARG, "mjx_train_bn_mish_fwd: bad arguments");
+    cudaStream_t s = (cudaStream_t)stream;
+    const int G = mjx_train::bn_blocks(rows), R = mjx_train::bn_rows_per_block(rows), C = channels;
+    const int threads = mjx_train::bn_lanes(C) * C;
+    MJX_TRAIN_DISPATCH(dtype, {
+        if (training) mjx_train::k_bn_stats<T><<<G, threads, 0, s>>>((const T*)x, rows, C, R, scratch);
+        mjx_train::k_bn_finalize<<<C, mjx_train::FIN_THREADS, 0, s>>>(scratch, G, C, rows, eps, momentum, training, running_mean,
+                                                                 running_var, save_mean, save_invstd);
+        const int n = rows * C;
+        mjx_train::k_bn_mish_apply<T><<<train_grid(n), 256, 0, s>>>((const T*)x, save_mean, save_invstd, gamma, beta, (T*)out, n, C);
+    });
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+int mjx_train_bn_mish_bwd(int dtype, const void* x, const void* dout, const float* gamma, const float* beta, const float* save_mean,
+                          const float* save_invstd, void* dx, float* dgamma, float* dbeta, int rows, int channels, int training,
+                          float* scratch, void* stream) {
+    if (!train_shape_ok(dtype, rows, channels) || !x || !dout || !gamma || !beta || !save_mean || !save_invstd || !dx || !dgamma ||
+        !dbeta || !scratch || (uintptr_t)scratch % 8)
+        return fail(MJX_ERR_ARG, "mjx_train_bn_mish_bwd: bad arguments (scratch 8-byte aligned)");
+    cudaStream_t s = (cudaStream_t)stream;
+    const int G = mjx_train::bn_blocks(rows), R = mjx_train::bn_rows_per_block(rows), C = channels;
+    const int threads = mjx_train::bn_lanes(C) * C;
+    double* part = (double*)scratch;      // 2 * G * C doubles = the 4 * G * C floats the forward's partials take
+    float* coef = scratch + 4LL * G * C;  // after the partials
+    MJX_TRAIN_DISPATCH(dtype, {
+        mjx_train::k_bn_mish_bwd_sums<T><<<G, threads, 0, s>>>((const T*)x, (const T*)dout, save_mean, save_invstd, gamma, beta, rows,
+                                                               C, R, part);
+        mjx_train::k_bn_bwd_finalize<<<C, mjx_train::FIN_THREADS, 0, s>>>(part, G, C, rows, training, gamma, save_invstd, dgamma,
+                                                                     dbeta, coef);
+        const int n = rows * C;
+        mjx_train::k_bn_mish_bwd_dx<T><<<train_grid(n), 256, 0, s>>>((const T*)x, (const T*)dout, save_mean, save_invstd, gamma,
+                                                                     beta, coef, (T*)dx, n, C);
+    });
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+int mjx_train_gate_pool(int dtype, const void* y, void* avg, void* mx, int batch, int length, int channels, void* stream) {
+    if (!train_shape_ok(dtype, batch, channels, length) || !y || !avg || !mx)
+        return fail(MJX_ERR_ARG, "mjx_train_gate_pool: bad arguments");
+    MJX_TRAIN_DISPATCH(dtype, mjx_train::k_gate_pool<T><<<(batch * channels + 255) / 256, 256, 0, (cudaStream_t)stream>>>(
+                                  (const T*)y, (T*)avg, (T*)mx, batch, length, channels));
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+int mjx_train_gate_out(int dtype, const void* y, const void* g, const void* x, void* out, int batch, int length, int channels,
+                       void* stream) {
+    if (!train_shape_ok(dtype, batch, channels, length) || !y || !g || !x || !out)
+        return fail(MJX_ERR_ARG, "mjx_train_gate_out: bad arguments");
+    const int n = batch * length * channels;
+    MJX_TRAIN_DISPATCH(dtype, mjx_train::k_gate_out<T><<<train_grid(n), 256, 0, (cudaStream_t)stream>>>(
+                                  (const T*)y, (const T*)g, (const T*)x, (T*)out, n, length * channels, channels));
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+int mjx_train_gate_bwd_dg(int dtype, const void* dout, const void* y, const void* mx, float* dg, float* cnt, int batch, int length,
+                          int channels, void* stream) {
+    if (!train_shape_ok(dtype, batch, channels, length) || !dout || !y || !mx || !dg || !cnt)
+        return fail(MJX_ERR_ARG, "mjx_train_gate_bwd_dg: bad arguments");
+    MJX_TRAIN_DISPATCH(dtype, mjx_train::k_gate_bwd_dg<T><<<(batch * channels + 255) / 256, 256, 0, (cudaStream_t)stream>>>(
+                                  (const T*)dout, (const T*)y, (const T*)mx, dg, cnt, batch, length, channels));
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+int mjx_train_gate_bwd_dy(int dtype, const void* dout, const void* y, const void* g, const void* mx, const float* cnt,
+                          const void* davg, const void* dmx, void* dy, int batch, int length, int channels, void* stream) {
+    if (!train_shape_ok(dtype, batch, channels, length) || !dout || !y || !g || !mx || !cnt || !davg || !dmx || !dy)
+        return fail(MJX_ERR_ARG, "mjx_train_gate_bwd_dy: bad arguments");
+    const int n = batch * length * channels;
+    MJX_TRAIN_DISPATCH(dtype, mjx_train::k_gate_bwd_dy<T><<<train_grid(n), 256, 0, (cudaStream_t)stream>>>(
+                                  (const T*)dout, (const T*)y, (const T*)g, (const T*)mx, cnt, (const T*)davg, (const T*)dmx, (T*)dy,
+                                  n, length, channels));
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+int mjx_train_dqn_loss_fwd(int dtype, const void* v, const void* a, const uint8_t* masks, const int64_t* actions,
+                           const int64_t* steps_to_done, const double* rewards, const void* aux, const int64_t* ranks, int batch,
+                           int n_aux, float gamma, float* q_out, float* q_act, float* q_target, float* losses, int* bad,
+                           void* stream) {
+    if ((dtype != MJX_TRAIN_F32 && dtype != MJX_TRAIN_F16) || batch <= 0 || n_aux <= 0 || n_aux > 32 || !v || !a || !masks ||
+        !actions || !steps_to_done || !rewards || !aux || !ranks || !q_act || !q_target || !losses || !bad)
+        return fail(MJX_ERR_ARG, "mjx_train_dqn_loss_fwd: bad arguments");
+    MJX_TRAIN_DISPATCH(dtype, mjx_train::k_dqn_loss_fwd<T><<<1, mjx_train::LOSS_THREADS, 0, (cudaStream_t)stream>>>(
+                                  (const T*)v, (const T*)a, masks, actions, steps_to_done, rewards, (const T*)aux, ranks, batch, n_aux,
+                                  gamma, q_out, q_act, q_target, losses, bad));
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+int mjx_train_dqn_loss_bwd(int dtype, const void* v, const void* a, const uint8_t* masks, const int64_t* actions,
+                           const float* q_target, const void* aux, const int64_t* ranks, int batch, int n_aux, const float* w,
+                           void* dv, void* da, void* daux, void* stream) {
+    if ((dtype != MJX_TRAIN_F32 && dtype != MJX_TRAIN_F16) || batch <= 0 || n_aux <= 0 || n_aux > 32 || !v || !a || !masks ||
+        !actions || !q_target || !aux || !ranks || !w || !dv || !da || !daux)
+        return fail(MJX_ERR_ARG, "mjx_train_dqn_loss_bwd: bad arguments");
+    const long long blocks = ((long long)batch * 32 + 255) / 256;
+    MJX_TRAIN_DISPATCH(dtype, mjx_train::k_dqn_loss_bwd<T><<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(
+                                  (const T*)v, (const T*)a, masks, actions, q_target, (const T*)aux, ranks, batch, n_aux, w, (T*)dv,
+                                  (T*)da, (T*)daux));
+    CU(cudaGetLastError());
     return MJX_OK;
 }
 

@@ -9,7 +9,9 @@ observation concatenated along the channels. DQN heads: version 4 Linear(1024, 1
 heads (hidden 512 / 256); version 1 Linear heads on the 512-wide latent; the advantage mean is taken over legal actions only and
 illegal actions are -inf.
 
-The modules use their own parameter names; `load_mortal` is the one place that knows the reference's checkpoint key layout.
+The modules use their own parameter names; `_reference_prefixes` is the one place that knows the reference's checkpoint key
+layout, which `load_mortal`, `load_mortal_state` and `mortal_state_dict` share. `AuxNet` is the trainer's next-rank head
+(mortal/model.py:188-195); `Brain.forward_train` is the training forward on the fused kernels of mortal_b200.train_ops.
 """
 from __future__ import annotations
 
@@ -135,6 +137,47 @@ class Brain(nn.Module):
             self.latent = nn.Linear(1024, 512)
             self.mu_head = nn.Linear(512, 512)
             self.logsig_head = nn.Linear(512, 512)
+
+    def train(self, mode: bool = True):
+        """nn.Module.train, after which every BatchNorm1d stays in eval mode while the batch norms are frozen
+        (mortal/model.py:169-186)"""
+        super().train(mode)
+        if getattr(self, "_freeze_bn", False):
+            for mod in self.modules():
+                if isinstance(mod, nn.BatchNorm1d):
+                    mod.eval()
+        return self
+
+    def reset_running_stats(self):
+        for mod in self.modules():
+            if isinstance(mod, nn.BatchNorm1d):
+                mod.reset_running_stats()
+
+    def freeze_bn(self, value: bool):
+        self._freeze_bn = bool(value)
+        return self.train(self.training)
+
+    def forward_train(self, obs):
+        """phi [B, 1024] of versions 2-4 as `forward` computes it, for training: the convolutions are cuDNN on channels-last (1 x 3)
+        views of the Conv1d weights, every BatchNorm + Mish of the trunk and every channel gate + residual run as the fused
+        kernels of mortal_b200.train_ops (float32, or float16 under torch.autocast). Gradients reach this module's own parameters;
+        the BatchNorms update their running statistics when in train mode (not frozen), as `forward` does."""
+        from . import train_ops
+
+        if self.version == 1:
+            raise ValueError("forward_train: version 1 returns (mu, logsig), which mortal/train.py cannot train either")
+        if self.is_oracle:
+            raise ValueError("forward_train: oracle brains are not supported (mortal/train.py never passes invisible_obs)")
+        F = torch.nn.functional
+        train_ops.check_channels(self.stem.weight.shape[0])
+        w = lambda conv: conv.weight.unsqueeze(2)  # [Cout, Cin, 1, 3] view: autograd gives the Conv1d weight's gradient
+        x = F.conv2d(obs.unsqueeze(2).contiguous(memory_format=torch.channels_last), w(self.stem), padding=(0, 1))
+        for blk in self.blocks:
+            y = F.conv2d(train_ops.bn_mish(x, blk.bn1), w(blk.conv1), padding=(0, 1))
+            y = F.conv2d(train_ops.bn_mish(y, blk.bn2), w(blk.conv2), padding=(0, 1))
+            x = train_ops.gate_residual(y, x, blk.gate)
+        x = F.mish(F.conv2d(train_ops.bn_mish(x, self.bn), w(self.neck), self.neck.bias, padding=(0, 1)))
+        return F.mish(self.fc(x.flatten(1)))
 
     def forward(self, obs, invisible_obs=None):
         """phi [B, 1024] for versions 2-4, (mu, logsig) [B, 512] each for version 1, as mortal/model.py Brain.forward"""
@@ -264,13 +307,29 @@ class DQN(nn.Module):
             self.v_head = nn.Sequential(nn.Linear(1024, hidden), nn.Mish(inplace=True), nn.Linear(hidden, 1))
             self.a_head = nn.Sequential(nn.Linear(1024, hidden), nn.Mish(inplace=True), nn.Linear(hidden, ACTION_SPACE))
 
-    def forward(self, phi, mask):
+    def heads(self, phi):
+        """(v [B, 1], a [B, 46]) before the masked combine"""
         if self.version == 4:
-            v, a = self.net(phi).split((1, ACTION_SPACE), dim=-1)
-        else:
-            v, a = self.v_head(phi), self.a_head(phi)
+            return self.net(phi).split((1, ACTION_SPACE), dim=-1)
+        return self.v_head(phi), self.a_head(phi)
+
+    def forward(self, phi, mask):
+        v, a = self.heads(phi)
         a_mean = a.masked_fill(~mask, 0.0).sum(-1, keepdim=True) / mask.sum(-1, keepdim=True)
         return (v + a - a_mean).masked_fill(~mask, -torch.inf)
+
+
+class AuxNet(nn.Module):
+    """mortal/model.py:188-195: Linear(1024, sum(dims), bias=False) split by `dims`; the trainer's is AuxNet((4,)), the next-rank
+    logits"""
+
+    def __init__(self, dims=None):
+        super().__init__()
+        self.dims = dims
+        self.net = nn.Linear(1024, sum(dims), bias=False)
+
+    def forward(self, x):
+        return self.net(x).split(self.dims, dim=-1)
 
 
 class GRP(nn.Module):
@@ -315,15 +374,15 @@ def _reference_prefixes(brain: Brain) -> dict:
     return m
 
 
-def _load_strict(module: nn.Module, given: dict, rename, what: str):
+def _load_strict(module: nn.Module, given: dict, rename, what: str, batches_tracked: bool = False):
     """load `given` (reference key -> tensor) into `module`, whose key k is stored as rename(k): every key present with its
-    shape and nothing else; BatchNorm's num_batches_tracked is accepted and ignored"""
+    shape and nothing else; BatchNorm's num_batches_tracked is optional, and ignored unless `batches_tracked`"""
     own = module.state_dict()
     want = {rename(k): k for k in own}
     out = {}
     for rk, k in want.items():
         if k.endswith(".num_batches_tracked"):
-            out[k] = own[k]
+            out[k] = given[rk] if batches_tracked and rk in given else own[k]
             continue
         if rk not in given:
             raise KeyError(f"{what}: missing key {rk!r}")
@@ -335,6 +394,37 @@ def _load_strict(module: nn.Module, given: dict, rename, what: str):
     if extra:
         raise KeyError(f"{what}: unexpected key {extra[0]!r}")
     module.load_state_dict(out)
+
+
+def _reference_key(names: dict, k: str) -> str:
+    mod, leaf = k.rsplit(".", 1)
+    return names[mod] + "." + leaf
+
+
+# the registration order of the reference Brain's submodules (state_dict order): a name's rank among its siblings
+_REF_MODULE_RANK = {"latent_net": 0, "mu_head": 1, "logsig_head": 2, "encoder": 3, "net": 0, "res_unit": 0, "ca": 1, "shared_mlp": 0}
+_REF_LEAF_RANK = {"weight": 0, "bias": 1, "running_mean": 2, "running_var": 3, "num_batches_tracked": 4}
+
+
+def _reference_order(rk: str):
+    *mods, leaf = rk.split(".")
+    return [int(m) if m.isdigit() else _REF_MODULE_RANK[m] for m in mods], _REF_LEAF_RANK[leaf]
+
+
+def mortal_state_dict(brain: Brain) -> dict:
+    """brain.state_dict() under mortal/model.py's Brain keys (`encoder.net.*`, `latent_net.*`, ...) and in its order, the
+    BatchNorms' num_batches_tracked included: the `mortal` entry of a reference state file. The inverse of load_mortal_state."""
+    names = _reference_prefixes(brain)
+    ref = {_reference_key(names, k): v for k, v in brain.state_dict().items()}
+    return {rk: ref[rk] for rk in sorted(ref, key=_reference_order)}
+
+
+def load_mortal_state(brain: Brain, sd: dict, batches_tracked: bool = True):
+    """load a state dict in mortal/model.py's Brain key layout (mortal_state_dict's, a reference state file's `mortal`) into
+    `brain`, strictly: every key with its shape and nothing else. num_batches_tracked is optional; when given it is loaded
+    unless `batches_tracked` is False (load_mortal's inference brains ignore it)."""
+    names = _reference_prefixes(brain)
+    _load_strict(brain, sd, lambda k: _reference_key(names, k), "mortal", batches_tracked)
 
 
 def load_mortal(state: dict):
@@ -360,8 +450,7 @@ def load_mortal(state: dict):
     if blocks != n:
         raise ValueError(f"mortal: {blocks} residual blocks in the state dict, config resnet.num_blocks is {n}")
     brain = Brain(conv_channels=c, num_blocks=n, version=version, is_oracle=cin != OBS_ROWS[version])
-    names = _reference_prefixes(brain)
-    _load_strict(brain, sd, lambda k: names[k.rsplit(".", 1)[0]] + "." + k.rsplit(".", 1)[1], "mortal")
+    load_mortal_state(brain, sd, batches_tracked=False)
     dqn = DQN(version=version)
     _load_strict(dqn, state["current_dqn"], lambda k: k, "current_dqn")
     return brain.eval(), dqn.eval()
