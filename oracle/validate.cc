@@ -1,8 +1,8 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY (see mj.h).
 // Restates libriichi bin/validate_logs.rs:62-242 process_path over the oracle PlayerState: the checks of every event, then
 // update(ev, keep_cans_on_announce = true) for seats 0..3; the first failure ends the log.
-// Built with the other oracle sources (without capi.cc) into oracle/libvalidate.so by tests/validate_lib.py, which binds the C
-// entry points at the end of this file.
+// Part of oracle/liboracle.so; tests/validate_lib.py binds the C entry points at the end of this file. orcv_init loads the tables
+// for a library built from the oracle sources without capi.cc (in liboracle.so, orc_init has already loaded them).
 #include <algorithm>
 #include <memory>
 #include <string>

@@ -27,9 +27,9 @@ def main():
     ap.add_argument("--procs", type=int, default=os.cpu_count())
     ap.add_argument("--slices", type=int, default=4096)
     a = ap.parse_args()
-    import mjai_write_lib as W
+    import emul_lib
 
-    W.build()
+    emul_lib.build()
     step = (1 << 32) // a.slices
     parts = [(i * step, (i + 1) * step if i + 1 < a.slices else 1 << 32) for i in range(a.slices)]
     t0, bad, first = time.time(), 0, None

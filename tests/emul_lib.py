@@ -1,31 +1,48 @@
-"""ctypes binding of tests/host_emul/libmjx_emul.so — TEST INFRASTRUCTURE (single-lane host build of the
-product's step sources; see tests/host_emul/emul.cc). Never used by mortal_b200/."""
+"""Builds and binds tests/host_emul/libmjx_emul.so — TEST INFRASTRUCTURE: every tests/host_emul/*.cc (single-lane host builds
+of the product's device sources, -DMJX_HOST_EMUL) linked into one library. This module binds emul.cc's entries; the feature
+helpers (validate_lib, mjai_lib, ...) declare their own entries on lib(). Never used by mortal_b200/."""
 import ctypes as C
+import glob
 import os
 import subprocess
+import tempfile
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "host_emul", "emul.cc")
-SO = os.path.join(ROOT, "tests", "host_emul", "libmjx_emul.so")
+HOST_EMUL = os.path.join(ROOT, "tests", "host_emul")
+SO = os.path.join(HOST_EMUL, "libmjx_emul.so")
+ASAN_SO = os.path.join(HOST_EMUL, "libmjx_emul_asan.so")
 CSRC = os.path.join(ROOT, "mortal_b200", "csrc")
 DATA_DIR = os.path.join(ROOT, "mortal_b200", "data")
-_lib = None
+FLAGS = ["-g", "-std=c++17", "-fPIC", "-DMJX_HOST_EMUL", "-ffp-contract=off", "-Wall", "-Wno-unknown-pragmas", "-I" + CSRC]
+_lib = _pylib = None
 
 
-def build():
-    deps = [SRC] + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
-    if not os.path.exists(SO) or any(os.path.getmtime(d) > os.path.getmtime(SO) for d in deps):
-        subprocess.check_call(["g++", "-O2", "-g", "-std=c++17", "-fPIC", "-shared", "-DMJX_HOST_EMUL", "-ffp-contract=off", "-I" + CSRC,
-                               "-Wno-unknown-pragmas", "-o", SO, SRC])
-    return SO
+def build(sanitize=False):
+    """Compiles the library when it is older than a source, a csrc/ file, include/mjx.h or this file (the flags); returns its
+    path. sanitize=True builds the same sources under ASan + UBSan into a file of its own, so it never replaces the normal build."""
+    so = ASAN_SO if sanitize else SO
+    srcs = sorted(glob.glob(os.path.join(HOST_EMUL, "*.cc")))
+    deps = srcs + [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(ROOT, "include", "mjx.h"), __file__]
+    if os.path.exists(so) and all(os.path.getmtime(d) <= os.path.getmtime(so) for d in deps):
+        return so
+    opt = ["-O1", "-fsanitize=address,undefined", "-fno-omit-frame-pointer"] if sanitize else ["-O2"]
+    with tempfile.TemporaryDirectory() as tmp:  # one compiler per source, in parallel: emul.cc alone takes ~10 s
+        objs = [os.path.join(tmp, os.path.basename(s) + ".o") for s in srcs]
+        procs = [subprocess.Popen(["g++", *opt, *FLAGS, "-c", "-o", o, s]) for s, o in zip(srcs, objs)]
+        if [p.wait() for p in procs] != [0] * len(procs):
+            raise RuntimeError("compiling tests/host_emul failed")
+        subprocess.check_call(["g++", *opt, "-shared", "-Wl,--no-undefined", "-o", so, *objs])
+    return so
 
 
-def lib():
+def lib(sanitize=False):
+    """The library, loaded once, with emul.cc's entries bound and the lookup tables loaded. A sanitizer run calls
+    lib(sanitize=True) before anything else loads the library."""
     global _lib
     if _lib is None:
-        L = C.CDLL(build())
+        L = C.CDLL(build(sanitize))
         L.emul_last_error.restype = C.c_char_p
         L.emul_init.argtypes = [C.c_char_p]
         L.emul_shanten.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
@@ -58,10 +75,21 @@ def lib():
         L.emul_env_read_log.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         L.emul_env_log_lens.argtypes = [C.c_void_p, C.c_void_p]
         L.emul_env_results.argtypes = [C.c_void_p] + [C.c_void_p] * 5
+        L.emul_replay_viewpoints.argtypes = [C.c_void_p, C.c_void_p]
         if L.emul_init(DATA_DIR.encode()) != 0:
             raise RuntimeError(L.emul_last_error().decode())
         _lib = L
+    elif sanitize and _lib._name != ASAN_SO:
+        raise RuntimeError("libmjx_emul.so is already loaded without sanitizers")
     return _lib
+
+
+def pylib():
+    """lib()'s file loaded again with ctypes.PyDLL, whose calls hold the GIL: for entries that call back into Python"""
+    global _pylib
+    if _pylib is None:
+        _pylib = C.PyDLL(lib()._name)
+    return _pylib
 
 
 def run(nonces, keys, *, shuffle_kind=0, quick_eval=True, policy_kind=1, trace_cap=0, max_cycles=0, agari_guard=False):
@@ -192,6 +220,13 @@ class EmulReplay(EmulEnv):
         out = np.zeros((self.num_rows(), 211 if version == 1 else 217, 34), dtype=np.float32)
         self.L.emul_replay_encode_invisible(self._h, out.ctypes.data, version)
         return out
+
+    def viewpoints(self):
+        """mjx_env_replay_viewpoints / ReplayEnv.viewpoints(): single-viewpoint logs replay from the player's own seat; returns
+        the scan result per job (-1 = not marked, else the mask of hidden seats)"""
+        m = np.zeros(self.n_tables, dtype=np.int32)
+        self.L.emul_replay_viewpoints(self._h, m.ctypes.data)
+        return m
 
     def row_labels(self):
         n = self.num_rows()

@@ -5,7 +5,6 @@ from __future__ import annotations
 import ctypes as C
 import os
 import re
-import subprocess
 
 import numpy as np
 
@@ -14,9 +13,6 @@ import stat_lib as S
 from mortal_b200.dataset import Grp
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMUL_SRC = os.path.join(ROOT, "tests", "host_emul", "emul_grp.cc")
-EMUL_SO = os.path.join(ROOT, "tests", "host_emul", "libmjx_emul_grp.so")
-_emul = None
 
 
 def _statuses():
@@ -32,28 +28,12 @@ STATUS = _statuses()
 encode = S.encode
 
 
-def build_emul(so=EMUL_SO, extra=()):
-    deps = [EMUL_SRC, os.path.join(ROOT, "include", "mjx.h")] + [os.path.join(E.CSRC, f) for f in
-                                                                   ("mjx_grp.cuh", "mjx_mjai.cuh", "mjx_types.cuh", "mjx_port.cuh")]
-    if extra or not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
-        subprocess.check_call(["g++", "-O2" if not extra else "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-DMJX_HOST_EMUL",
-                               "-Wall", "-I" + E.CSRC, "-Wno-unknown-pragmas", *extra, "-o", so, EMUL_SRC])
-    return so
-
-
-def build():
-    build_emul()
-
-
-def emul_lib(path=None):
-    """the emulated kernel; `path` loads another build of emul_grp.cc (the sanitizer run's)"""
-    global _emul
-    if _emul is None or path is not None:
-        L = C.CDLL(path or build_emul())
-        L.emulg_grp_logs.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong,
-                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        _emul = L
-    return _emul
+def emul_lib():
+    """emul_lib.lib() with the emulated kernel's entry declared"""
+    L = E.lib()
+    L.emulg_grp_logs.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong,
+                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    return L
 
 
 def run_emul(a, n_hdr=None, n_kyoku_words=None):

@@ -5,9 +5,7 @@ GrpFileDatasetsIter over stub or real file lists."""
 from __future__ import annotations
 
 import ctypes as C
-import os
 import random
-import subprocess
 
 import numpy as np
 import torch
@@ -17,39 +15,17 @@ from torch.nn.utils.rnn import pack_padded_sequence, pad_sequence
 import emul_lib as E
 from reward_lib import RefGRP, random_feature, random_grp  # noqa: F401  (re-exported for the tests)
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMUL_SRC = os.path.join(ROOT, "tests", "host_emul", "emul_grp_train.cc")
-EMUL_SO = os.path.join(ROOT, "tests", "host_emul", "libmjx_emul_grp_train.so")
-_emul = None
 
-
-def build_emul(so=EMUL_SO, extra=()):
-    deps = [EMUL_SRC, os.path.join(ROOT, "include", "mjx.h")] + [os.path.join(E.CSRC, f) for f in
-                                                                   ("mjx_grp_train.cuh", "mjx_reward.cuh", "mjx_types.cuh",
-                                                                    "mjx_port.cuh")]
-    if extra or not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
-        subprocess.check_call(["g++", "-O2" if not extra else "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-DMJX_HOST_EMUL",
-                               "-Wall", "-I" + E.CSRC, "-Wno-unknown-pragmas", *extra, "-o", so, EMUL_SRC])
-    return so
-
-
-def build():
-    build_emul()
-
-
-def emul_lib(path=None):
-    """the emulated kernels; `path` loads another build of emul_grp_train.cc (the sanitizer run's)"""
-    global _emul
-    if _emul is None or path is not None:
-        L = C.CDLL(path or build_emul())
-        L.emult_grp_train.restype = C.c_int
-        L.emult_grp_train.argtypes = ([C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_int, C.c_int,
-                                       C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 5 + [C.c_int]
-                                      + [C.c_void_p] * 5 + [C.c_longlong])
-        L.emult_scratch_bytes.restype = C.c_longlong
-        L.emult_scratch_bytes.argtypes = [C.c_int] * 5
-        _emul = L
-    return _emul
+def emul_lib():
+    """emul_lib.lib() with the emulated kernels' entries declared"""
+    L = E.lib()
+    L.emult_grp_train.restype = C.c_int
+    L.emult_grp_train.argtypes = ([C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_int, C.c_int,
+                                   C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 5 + [C.c_int]
+                                  + [C.c_void_p] * 5 + [C.c_longlong])
+    L.emult_scratch_bytes.restype = C.c_longlong
+    L.emult_scratch_bytes.argtypes = [C.c_int] * 5
+    return L
 
 
 def pack(grp):

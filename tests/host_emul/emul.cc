@@ -1,6 +1,7 @@
-// TEST INFRASTRUCTURE ONLY — single-lane host build of mortal_b200/csrc/mjx_step.cuh (-DMJX_HOST_EMUL).
-// Lets the GPU-less dev container diff the product's rule logic against the oracle. Never loaded by
-// mortal_b200/; the product has no CPU path.
+// TEST INFRASTRUCTURE ONLY — single-lane host build of mortal_b200/csrc/mjx_step.cuh (-DMJX_HOST_EMUL), with the replay,
+// the single-viewpoint scan and the log validator (k_validate_logs). Lets the GPU-less dev container diff the product's rule
+// logic against the oracle. Never loaded by mortal_b200/; the product has no CPU path. Built by tests/emul_lib.py, which
+// also binds these entries; emul_init loads the lookup tables for all of them.
 #include <cstdint>
 #include <cstring>
 #include <string>
@@ -11,6 +12,7 @@
 #include "mjx_invisible.cuh"
 #include "mjx_state.cuh"
 #include "mjx_policy.cuh"
+#include "mjx_validate.cuh"
 #include "mjx_tables_host.h"
 
 using namespace mjx;
@@ -226,6 +228,17 @@ int emul_replay_step(void* p) {
         if (replay_table(c, E->V, E->R, t)) live++;
     }
     return live;
+}
+// mjx_env_replay_viewpoints on an emul_replay_create env: the scan and the mark, one lane per job; the scan result of every job
+// (-1 = not marked, else the mask of hidden seats) goes to `masks` when it is not null
+void emul_replay_viewpoints(void* p, int32_t* masks) {
+    EmulEnv* E = static_cast<EmulEnv*>(p);
+    const long long n_hdr = (long long)E->r_hdr.size(), n_kyoku = (long long)(E->r_kyoku.size() / REPLAY_KYOKU_WORDS);
+    for (int t = 0; t < E->n; t++) {
+        const int mask = replay_hidden_seats(E->R, t, n_hdr, n_kyoku, 0);
+        replay_mark_viewpoint(&E->tabs[t], E->R.player[t], mask);
+        if (masks) masks[t] = mask;
+    }
 }
 void emul_replay_rows(void* p, int64_t* labels, uint8_t* meta) {
     EmulEnv* E = static_cast<EmulEnv*>(p);
@@ -444,6 +457,30 @@ void emul_env_results(void* p, int32_t* scores, uint8_t* ranks, int32_t* steps, 
     memcpy(scores, E->scores.data(), sizeof(i32) * 4 * E->n); memcpy(ranks, E->ranks.data(), 4 * E->n);
     memcpy(steps, E->steps.data(), sizeof(i32) * E->n); memcpy(errs, E->errs.data(), sizeof(i32) * E->n);
     memcpy(done, E->done.data(), sizeof(i32) * E->n);
+}
+
+// ---- mjx_validate_logs one log at a time; the same argument checks as the C ABI, returns 0 or -2
+int emulv_validate_logs(int n_logs, const uint64_t* hdr, const int32_t* ev_off, const int32_t* ev_cnt, long long n_hdr,
+                        const uint64_t* kyoku, const int32_t* ky_off, long long n_kyoku_words, const uint64_t* hora,
+                        const int32_t* hora_off, long long n_hora_words, mjx_verdict* out) {
+    if (!g_ready || n_logs <= 0 || !ev_off || !ev_cnt || !ky_off || !hora_off || !out || n_hdr < 0 || (n_hdr > 0 && !hdr) ||
+        n_kyoku_words < 0 || n_kyoku_words % REPLAY_KYOKU_WORDS || (n_kyoku_words > 0 && !kyoku) || n_hora_words < 0 ||
+        n_hora_words % MJX_HORA_WORDS || (n_hora_words > 0 && !hora))
+        return -2;
+    for (int i = 0; i < n_logs; i++)
+        if (ev_off[i] < 0 || ev_cnt[i] < 0 || (long long)ev_off[i] + ev_cnt[i] > n_hdr || ky_off[i] < 0 || hora_off[i] < 0) return -2;
+    ValidateView V;
+    V.hdr = hdr; V.ev_off = ev_off; V.ev_cnt = ev_cnt; V.kyoku = kyoku; V.ky_off = ky_off; V.hora = hora; V.hora_off = hora_off;
+    V.n_kyoku = n_kyoku_words / REPLAY_KYOKU_WORDS; V.n_hora = n_hora_words / MJX_HORA_WORDS; V.n_logs = n_logs; V.out = out;
+    std::vector<TableState> rec(1);
+    WarpScratch W;
+    for (int i = 0; i < n_logs; i++) {
+        memset(rec.data(), 0, sizeof(TableState));
+        Ctx c;
+        c.S = rec.data(); c.W = &W; c.T = g_T; c.lane = 0; c.df = W.dora_factor;
+        validate_log(c, V, i);
+    }
+    return 0;
 }
 
 }  // extern "C"

@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY — single-lane host build of mortal_b200/csrc/mjx_grp.cuh (-DMJX_HOST_EMUL): the per-log walk of
 // k_grp_logs, so the GRP targets can be diffed against Grp.load_events and run under sanitizers without a GPU. Never loaded by
-// mortal_b200/. Built by tests/grp_lib.py.
+// mortal_b200/. Part of libmjx_emul.so (tests/emul_lib.py); bound by tests/grp_lib.py.
 #include <cstdint>
 
 #include "mjx_grp.cuh"

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY — host build of mortal_b200/csrc/mjx_grp_train.cuh (-DMJX_HOST_EMUL): the phase functions of
 // k_grp_train_fwd / head / bwd / wgrad / loss run for every thread id in turn between the barriers (one slice per dot product), so
 // the GRP training step can be diffed against a torch restatement of the reference and run under sanitizers without a GPU.
-// Never loaded by mortal_b200/. Built by tests/grp_train_lib.py.
+// Never loaded by mortal_b200/. Part of libmjx_emul.so (tests/emul_lib.py); bound by tests/grp_train_lib.py.
 #include <cstdint>
 #include <vector>
 

@@ -1,8 +1,8 @@
 // TEST INFRASTRUCTURE ONLY — host build of mortal_b200/csrc/mjx_mjai.cuh (-DMJX_HOST_EMUL): the line parser of k_mjai_decode
 // driven by a restatement of the kernel's warp walk (the same 128-byte steps, 32-byte windows, 64-entry queue of line ends and
 // 32-line flushes, the lanes run one after another), so the decoder's accept / decline rule, its arrays and its queue indexing
-// can be diffed against the Python decoder and run under sanitizers without a GPU. Never loaded by mortal_b200/. Built by
-// tests/mjai_lib.py.
+// can be diffed against the Python decoder and run under sanitizers without a GPU. Never loaded by mortal_b200/. Part of
+// libmjx_emul.so (tests/emul_lib.py); bound by tests/mjai_lib.py.
 #include <cstdint>
 #include <cstring>
 #include <vector>

@@ -2,7 +2,7 @@
 // per-event renderer of k_mjai_render driven by one host lane that walks a game's events in order (the kernel's lanes take 32
 // consecutive events at a time and place them by a prefix sum: the same events in the same order). Lets the renderer be diffed
 // against mortal_b200/mjai_log.py and CPython's float repr, and run under sanitizers, without a GPU. Never loaded by
-// mortal_b200/. Built by tests/mjai_write_lib.py.
+// mortal_b200/. Part of libmjx_emul.so (tests/emul_lib.py); bound by tests/mjai_write_lib.py.
 #include <cmath>
 #include <cstdint>
 #include <cstring>

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY — host build of the training-buffer observation codec (mortal_b200/csrc/mjx_obs_pack.cuh, the record
 // layout of csrc/mjx_obs.cuh make_obs_record, -DMJX_HOST_EMUL): k_obs_pack's work one sample at a time and k_obs_unpack's through
 // the host enc_materialize, slice by slice, so the codec can be checked on oracle observations and run under sanitizers without a
-// GPU. Never loaded by mortal_b200/. Built by tests/obs_pack_lib.py.
+// GPU. Never loaded by mortal_b200/. Part of libmjx_emul.so (tests/emul_lib.py); bound by tests/obs_pack_lib.py.
 #include <cstdint>
 #include <cstring>
 

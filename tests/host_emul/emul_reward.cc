@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY — host build of mortal_b200/csrc/mjx_reward.cuh (-DMJX_HOST_EMUL): k_grp_matrix's phase functions
 // run for every thread id in turn between the barriers (one slice per dot product), and k_train_targets's per-job work for one
 // lane, so the GRP rewards can be diffed against a torch restatement of the reference and run under sanitizers without a GPU.
-// Never loaded by mortal_b200/. Built by tests/reward_lib.py.
+// Never loaded by mortal_b200/. Part of libmjx_emul.so (tests/emul_lib.py); bound by tests/reward_lib.py.
 #include <cstdint>
 #include <vector>
 

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY — single-lane host build of mortal_b200/csrc/mjx_stat.cuh (-DMJX_HOST_EMUL): the per-log walk of
 // k_stat_logs with one lane playing all four seats, and the decoder's deltas reader (mjai_line_deltas of csrc/mjx_mjai.cuh), so
 // the statistics can be diffed against Stat.from_game and run under sanitizers without a GPU. Never loaded by mortal_b200/.
-// Built by tests/stat_lib.py.
+// Part of libmjx_emul.so (tests/emul_lib.py); bound by tests/stat_lib.py.
 #include <cstdint>
 #include <cstring>
 

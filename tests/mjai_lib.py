@@ -6,7 +6,6 @@ from __future__ import annotations
 import ctypes as C
 import json
 import os
-import subprocess
 
 import numpy as np
 
@@ -15,33 +14,14 @@ from mortal_b200 import dataset_codec
 from mortal_b200.validate_logs import EncodedLog, encode_log
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMUL_SRC = os.path.join(ROOT, "tests", "host_emul", "emul_mjai.cc")
-EMUL_SO = os.path.join(ROOT, "tests", "host_emul", "libmjx_emul_mjai.so")
-_emul = None
 
 
-def build_emul(so=EMUL_SO, extra=()):
-    deps = [EMUL_SRC, os.path.join(ROOT, "include", "mjx.h"), os.path.join(E.CSRC, "mjx_mjai.cuh"), os.path.join(E.CSRC, "mjx_types.cuh"),
-            os.path.join(E.CSRC, "mjx_port.cuh")]
-    if extra or not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
-        subprocess.check_call(["g++", "-O2" if not extra else "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-DMJX_HOST_EMUL",
-                               "-Wall", "-I" + E.CSRC, "-Wno-unknown-pragmas", *extra, "-o", so, EMUL_SRC])
-    return so
-
-
-def build():
-    build_emul()
-
-
-def emul_lib(path=None):
-    """the emulated decoder; `path` loads another build of emul_mjai.cc (the sanitizer run's)"""
-    global _emul
-    if _emul is None or path is not None:
-        L = C.CDLL(path or build_emul())
-        L.emulm_decode.argtypes = [C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
-                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong]
-        _emul = L
-    return _emul
+def emul_lib():
+    """emul_lib.lib() with the emulated decoder's entry declared"""
+    L = E.lib()
+    L.emulm_decode.argtypes = [C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong]
+    return L
 
 
 def emul_decode(blobs, augment=False):

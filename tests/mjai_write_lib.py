@@ -3,54 +3,36 @@ emul_mjai_write.cc), its bindings, and the comparison against CPython's float re
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "mortal_b200", "csrc")
-EMUL_SRC = os.path.join(ROOT, "tests", "host_emul", "emul_mjai_write.cc")
-EMUL_SO = os.path.join(ROOT, "tests", "host_emul", "libmjx_emul_mjai_write.so")
-_emul = None
+import emul_lib as E
 
 
-def build_emul(so=EMUL_SO, extra=()):
-    deps = [EMUL_SRC, os.path.join(ROOT, "include", "mjx.h"), os.path.join(CSRC, "mjx_mjai_write.cuh"),
-            os.path.join(CSRC, "mjx_types.cuh"), os.path.join(CSRC, "mjx_port.cuh")]
-    if extra or not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
-        subprocess.check_call(["g++", "-O2" if not extra else "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-DMJX_HOST_EMUL",
-                               "-Wall", "-I" + CSRC, "-Wno-unknown-pragmas", *extra, "-o", so, EMUL_SRC])
-    return so
+def emul_lib():
+    """emul_lib.lib() with the emulated writer's entries declared"""
+    L = E.lib()
+    L.emulw_format_f32.restype = C.c_longlong
+    L.emulw_format_f32.argtypes = [C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong]
+    L.emulw_render.restype = C.c_int
+    L.emulw_render.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                               C.c_longlong]
+    L.emulw_meta_record.restype = C.c_int
+    L.emulw_meta_record.argtypes = ([C.c_longlong] + [C.c_void_p] * 4 + [C.c_int, C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_int]
+                                    + [C.c_void_p] * 7 + [C.c_longlong, C.c_longlong])
+    return L
 
 
-def build():
-    build_emul()
-
-
-def emul_lib(path=None):
-    """the emulated writer, loaded with ctypes.PyDLL: emulw_sweep calls back into this interpreter and needs the GIL held;
-    `path` loads another build of emul_mjai_write.cc (the sanitizer run's)"""
-    global _emul
-    if _emul is None or path is not None:
-        L = C.PyDLL(path or build_emul())
-        L.emulw_format_f32.restype = C.c_longlong
-        L.emulw_format_f32.argtypes = [C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong]
-        L.emulw_sweep.restype = C.c_longlong
-        L.emulw_sweep.argtypes = [C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
-        L.emulw_check.restype = C.c_longlong
-        L.emulw_check.argtypes = [C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
-        L.emulw_render.restype = C.c_int
-        L.emulw_render.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
-                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                   C.c_longlong]
-        L.emulw_meta_record.restype = C.c_int
-        L.emulw_meta_record.argtypes = ([C.c_longlong] + [C.c_void_p] * 4 + [C.c_int, C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_int]
-                                        + [C.c_void_p] * 7 + [C.c_longlong, C.c_longlong])
-        if path is not None:
-            return L
-        _emul = L
-    return _emul
+def callback_lib():
+    """emul_lib.pylib() with the formatter's comparison entries declared: they call back into this interpreter
+    (PyOS_double_to_string) and need the GIL held"""
+    L = E.pylib()
+    L.emulw_sweep.restype = C.c_longlong
+    L.emulw_sweep.argtypes = [C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
+    L.emulw_check.restype = C.c_longlong
+    L.emulw_check.argtypes = [C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
+    return L
 
 
 def format_f32(values) -> list[str]:
@@ -67,28 +49,26 @@ def _py_fns():
     return C.cast(C.pythonapi.PyOS_double_to_string, C.c_void_p).value, C.cast(C.pythonapi.PyMem_Free, C.c_void_p).value
 
 
-def sweep(lo: int, hi: int, step: int = 1, lib=None):
+def sweep(lo: int, hi: int, step: int = 1):
     """(mismatches, first mismatching bit pattern) of the formatter against PyOS_double_to_string over [lo, hi)"""
-    L = lib or emul_lib()
     first = C.c_uint64(0)
-    n = L.emulw_sweep(lo, hi, step, *_py_fns(), C.byref(first))
+    n = callback_lib().emulw_sweep(lo, hi, step, *_py_fns(), C.byref(first))
     return int(n), int(first.value)
 
 
-def check(bits, lib=None):
+def check(bits):
     """(mismatches, first mismatching bit pattern) of the formatter against PyOS_double_to_string over a list of patterns"""
-    L = lib or emul_lib()
     bits = np.ascontiguousarray(bits, dtype=np.uint32)
     first = C.c_uint64(0)
-    n = L.emulw_check(bits.ctypes.data, len(bits), *_py_fns(), C.byref(first))
+    n = callback_lib().emulw_check(bits.ctypes.data, len(bits), *_py_fns(), C.byref(first))
     return int(n), int(first.value)
 
 
-def render(words, lens, bounds=None, recs=None, lib=None):
+def render(words, lens, bounds=None, recs=None):
     """the emulated count + fill over host arrays: (status int32 [n_games], list of text bytes per game (None: non-zero status))"""
     from mortal_b200 import mjai_write
 
-    L = lib or emul_lib()
+    L = emul_lib()
     words = np.ascontiguousarray(words, dtype=np.uint64)
     lens = np.ascontiguousarray(lens, dtype=np.int32)
     n, cap = words.shape
@@ -109,8 +89,8 @@ def render(words, lens, bounds=None, recs=None, lib=None):
 class EmulRecords:
     """DeviceMetaRecorder's record arrays on the host, appended by the host build of k_meta_record (emulw_meta_record)"""
 
-    def __init__(self, cap, lib=None):
-        self.L = lib or emul_lib()
+    def __init__(self, cap):
+        self.L = emul_lib()
         self.cap, self.count, self.calls, self.max_cycle = cap, 0, [], -1
         self.table, self.cycle = np.zeros(cap, np.int32), np.zeros(cap, np.int32)
         self.seat, self.info = np.zeros(cap, np.uint8), np.zeros((cap, 4), np.int32)

@@ -4,48 +4,28 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 
 import emul_lib as E
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMUL_SRC = os.path.join(ROOT, "tests", "host_emul", "emul_obs_pack.cc")
-EMUL_SO = os.path.join(ROOT, "tests", "host_emul", "libmjx_emul_obs_pack.so")
 ROWS = {(1, False): 938, (2, False): 942, (3, False): 934, (4, False): 1012, (1, True): 211, (2, True): 217, (3, True): 217,
         (4, True): 217}
-_emul = None
 
 
-def build_emul(so=EMUL_SO, extra=()):
-    deps = [EMUL_SRC, os.path.join(ROOT, "include", "mjx.h")] + [os.path.join(E.CSRC, f) for f in os.listdir(E.CSRC)
-                                                                   if f.endswith((".cuh", ".h"))]
-    if extra or not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
-        subprocess.check_call(["g++", "-O2" if not extra else "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-DMJX_HOST_EMUL",
-                               "-ffp-contract=off", "-Wall", "-I" + E.CSRC, "-Wno-unknown-pragmas", *extra, "-o", so, EMUL_SRC])
-    return so
-
-
-def build():
-    build_emul()
-
-
-def emul_lib(path=None):
-    """the emulated codec; `path` loads another build of emul_obs_pack.cc (the sanitizer run's)"""
-    global _emul
-    if _emul is None or path is not None:
-        L = C.CDLL(path or build_emul())
-        L.emulp_record_bytes.restype = C.c_int
-        L.emulp_record_bytes.argtypes = [C.c_int, C.c_int]
-        L.emulp_pack.restype = C.c_int
-        L.emulp_pack.argtypes = [C.c_int, C.c_int, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p]
-        L.emulp_unpack.restype = C.c_int
-        L.emulp_unpack.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p]
-        L.emulp_value_rows.restype = C.c_int
-        L.emulp_value_rows.argtypes = [C.c_int, C.c_int, C.c_void_p]
-        _emul = L
-    return _emul
+def emul_lib():
+    """emul_lib.lib() with the emulated codec's entries declared"""
+    L = E.lib()
+    L.emulp_record_bytes.restype = C.c_int
+    L.emulp_record_bytes.argtypes = [C.c_int, C.c_int]
+    L.emulp_pack.restype = C.c_int
+    L.emulp_pack.argtypes = [C.c_int, C.c_int, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p]
+    L.emulp_unpack.restype = C.c_int
+    L.emulp_unpack.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p]
+    L.emulp_value_rows.restype = C.c_int
+    L.emulp_value_rows.argtypes = [C.c_int, C.c_int, C.c_void_p]
+    return L
 
 
 def record_bytes(version, invisible):

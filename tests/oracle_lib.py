@@ -135,7 +135,8 @@ _lib = None
 
 def build(force: bool = False) -> str:
     so = os.path.join(ORACLE_DIR, "liboracle.so")
-    srcs = [os.path.join(ORACLE_DIR, f) for f in os.listdir(ORACLE_DIR) if f.endswith((".cc", ".h"))]
+    srcs = [os.path.join(ORACLE_DIR, f) for f in os.listdir(ORACLE_DIR) if f.endswith((".cc", ".h"))] + \
+        [os.path.join(ROOT, "include", "mjx.h")]
     if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
         subprocess.check_call(["make", "-C", ORACLE_DIR, "liboracle.so"], stdout=subprocess.DEVNULL)
     return so

@@ -5,8 +5,6 @@ dataloader.py populate_buffer."""
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 from itertools import permutations
 
 import numpy as np
@@ -16,36 +14,15 @@ from torch.nn.utils.rnn import pack_padded_sequence, pad_sequence
 
 import emul_lib as E
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMUL_SRC = os.path.join(ROOT, "tests", "host_emul", "emul_reward.cc")
-EMUL_SO = os.path.join(ROOT, "tests", "host_emul", "libmjx_emul_reward.so")
-_emul = None
 
-
-def build_emul(so=EMUL_SO, extra=()):
-    deps = [EMUL_SRC, os.path.join(ROOT, "include", "mjx.h")] + [os.path.join(E.CSRC, f) for f in
-                                                                   ("mjx_reward.cuh", "mjx_types.cuh", "mjx_port.cuh")]
-    if extra or not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
-        subprocess.check_call(["g++", "-O2" if not extra else "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-DMJX_HOST_EMUL",
-                               "-Wall", "-I" + E.CSRC, "-Wno-unknown-pragmas", *extra, "-o", so, EMUL_SRC])
-    return so
-
-
-def build():
-    build_emul()
-
-
-def emul_lib(path=None):
-    """the emulated kernels; `path` loads another build of emul_reward.cc (the sanitizer run's)"""
-    global _emul
-    if _emul is None or path is not None:
-        L = C.CDLL(path or build_emul())
-        L.emulr_grp_reward.restype = C.c_int
-        L.emulr_grp_reward.argtypes = ([C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_int, C.c_int,
-                                        C.c_void_p, C.c_int, C.c_void_p, C.c_longlong] + [C.c_void_p] * 8 + [C.c_int]
-                                       + [C.c_void_p] * 4)
-        _emul = L
-    return _emul
+def emul_lib():
+    """emul_lib.lib() with the emulated kernels' entry declared"""
+    L = E.lib()
+    L.emulr_grp_reward.restype = C.c_int
+    L.emulr_grp_reward.argtypes = ([C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_int, C.c_int,
+                                    C.c_void_p, C.c_int, C.c_void_p, C.c_longlong] + [C.c_void_p] * 8 + [C.c_int]
+                                   + [C.c_void_p] * 4)
+    return L
 
 
 # ---------------------------------------------------------------- the reference, restated

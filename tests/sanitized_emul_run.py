@@ -2,15 +2,13 @@
 """Runs the product's rule / encoder / single-player / replay logic (the csrc/*.cuh sources, single-lane emulation build) under
 AddressSanitizer + UBSan. Usage (not part of the pytest suite; takes ~1 minute):
 
-    g++ -O1 -g -std=c++17 -fPIC -shared -DMJX_HOST_EMUL -ffp-contract=off -fsanitize=address,undefined -fno-omit-frame-pointer \
-        -Imortal_b200/csrc -o /tmp/libmjx_emul_asan.so tests/host_emul/emul.cc
     LD_PRELOAD=$(gcc -print-file-name=libasan.so):$(gcc -print-file-name=libubsan.so) ASAN_OPTIONS=detect_leaks=0 \
         python tests/sanitized_emul_run.py
 """
 import sys, numpy as np
 import os; ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, os.path.join(ROOT, 'tests')); sys.path.insert(0, ROOT)
 import emul_lib as E
-E.build = lambda force=False: '/tmp/libmjx_emul_asan.so'   # load the sanitised build instead
+E.lib(sanitize=True)
 from mortal_b200 import mjai_log, dataset_codec as DC
 # 1. self-play with logging, both policies
 for pol in (1, 0):

@@ -10,19 +10,18 @@ host. Usage (not part of the pytest suite):
 import json
 import os
 import sys
-import tempfile
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, ROOT)
+import emul_lib as E
 import grp_lib as G
 import log_mutations as LM
 import validate_lib as VL
 
-so = os.path.join(tempfile.mkdtemp(), "libmjx_emul_grp_asan.so")
-G.emul_lib(G.build_emul(so, extra=("-fsanitize=address,undefined", "-fno-omit-frame-pointer")))
+E.lib(sanitize=True)
 rng = np.random.default_rng(41)
 games = VL.emul_games(8, 1) + VL.emul_games(8, 0, seed0=6100)
 logs = list(games)

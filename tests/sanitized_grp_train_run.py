@@ -9,7 +9,6 @@ argument checks must refuse), so an out-of-range read or write shows on the host
 """
 import os
 import sys
-import tempfile
 
 import numpy as np
 import torch
@@ -17,10 +16,10 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, ROOT)
+import emul_lib as E
 import grp_train_lib as T
 
-so = os.path.join(tempfile.mkdtemp(), "libmjx_emul_grp_train_asan.so")
-T.emul_lib(T.build_emul(so, extra=("-fsanitize=address,undefined", "-fno-omit-frame-pointer")))
+E.lib(sanitize=True)
 rng = np.random.default_rng(47)
 
 # valid runs: several shape classes, compared with the reference

@@ -8,18 +8,17 @@ identically), so an out-of-range read on hostile text shows on the host. Usage (
 """
 import os
 import sys
-import tempfile
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, ROOT)
+import emul_lib as E
 import mjai_lib as M
 import validate_lib as VL
 
-so = os.path.join(tempfile.mkdtemp(), "libmjx_emul_mjai_asan.so")
-M.emul_lib(M.build_emul(so, extra=("-fsanitize=address,undefined", "-fno-omit-frame-pointer")))
+E.lib(sanitize=True)
 rng = np.random.default_rng(31)
 games = VL.emul_games(8, 1) + VL.emul_games(8, 0, seed0=5000)
 texts = [M.game_text(g) for g in games] + [M.vary(g, rng) for g in games]

@@ -9,19 +9,17 @@ Usage (not part of the pytest suite):
 """
 import os
 import sys
-import tempfile
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, ROOT)
+import emul_lib as E  # noqa: E402
 import mjai_write_lib as W  # noqa: E402
 import test_emul_mjai_write as T  # noqa: E402
 
-so = os.path.join(tempfile.mkdtemp(), "libmjx_emul_mjai_write_asan.so")
-lib = W.emul_lib(W.build_emul(so, extra=("-fsanitize=address,undefined", "-fno-omit-frame-pointer")))
-W._emul = lib
+E.lib(sanitize=True)
 rng = np.random.default_rng(41)
 for version in (4, 0):
     words, lens, rec = T.synthetic_batch(6, version, rng)
@@ -52,7 +50,7 @@ print(f"sanitised renderer run finished: 400 hostile batches, {hostile} games wi
 bad_rows = 0
 for trial in range(200):
     row_cap, n, cap = int(rng.integers(1, 40)), int(rng.integers(1, 60)), int(rng.integers(1, 80))
-    recs = W.EmulRecords(cap, lib=lib)
+    recs = W.EmulRecords(cap)
     recs.count = int(rng.integers(0, cap))
     idx = rng.integers(-5, row_cap + 5, size=n)
     masks = rng.integers(0, 2, size=(row_cap, 46))

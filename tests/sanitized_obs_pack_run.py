@@ -9,17 +9,16 @@ arguments the checks must refuse, so an out-of-range read or write shows on the 
 """
 import os
 import sys
-import tempfile
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, ROOT)
+import emul_lib as E
 import obs_pack_lib as P
 
-so = os.path.join(tempfile.mkdtemp(), "libmjx_emul_obs_pack_asan.so")
-P.emul_lib(P.build_emul(so, extra=("-fsanitize=address,undefined", "-fno-omit-frame-pointer")))
+E.lib(sanitize=True)
 rng = np.random.default_rng(47)
 bits = lambda a: np.ascontiguousarray(a).view(np.int32)
 hostile = np.array([0.5, -0.0, np.nan, 2.0, 1e-45, -1e-40, np.inf, -1.0], dtype=np.float32)

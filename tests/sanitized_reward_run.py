@@ -9,17 +9,16 @@ must refuse), so an out-of-range read or write shows on the host. Usage (not par
 """
 import os
 import sys
-import tempfile
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, ROOT)
+import emul_lib as E
 import reward_lib as R
 
-so = os.path.join(tempfile.mkdtemp(), "libmjx_emul_reward_asan.so")
-R.emul_lib(R.build_emul(so, extra=("-fsanitize=address,undefined", "-fno-omit-frame-pointer")))
+E.lib(sanitize=True)
 rng = np.random.default_rng(43)
 
 # valid runs: every shape class, compared with the reference

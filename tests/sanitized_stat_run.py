@@ -10,19 +10,18 @@ decoder's deltas reader over byte-mutated hora and ryukyoku lines. Usage (not pa
 import json
 import os
 import sys
-import tempfile
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, ROOT)
+import emul_lib as E
 import log_mutations as LM
 import stat_lib as S
 import validate_lib as VL
 
-so = os.path.join(tempfile.mkdtemp(), "libmjx_emul_stat_asan.so")
-S.emul_lib(S.build_emul(so, extra=("-fsanitize=address,undefined", "-fno-omit-frame-pointer")))
+E.lib(sanitize=True)
 rng = np.random.default_rng(37)
 games = VL.emul_games(8, 1) + VL.emul_games(8, 0, seed0=6000)
 logs = list(games)

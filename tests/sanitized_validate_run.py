@@ -9,19 +9,18 @@ the host that hostile input is rejected before the device sees it. Usage (not pa
 import json
 import os
 import sys
-import tempfile
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, ROOT)
+import emul_lib as E
 import log_mutations as LM
 import validate_lib as VL
 from mortal_b200.validate_logs import encode_log
 
-so = os.path.join(tempfile.mkdtemp(), "libmjx_emul_validate_asan.so")
-VL.emul_lib(VL.build_emul(so, extra=("-fsanitize=address,undefined", "-fno-omit-frame-pointer")))
+E.lib(sanitize=True)
 games = VL.emul_games(16, 1) + VL.emul_games(16, 0, seed0=5000)
 corpus = LM.mutated_corpus(games, 10, np.random.default_rng(11))
 assert VL.emul_validate([t for _, t in corpus]) == [VL.oracle_validate(t) for _, t in corpus]

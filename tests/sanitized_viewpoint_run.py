@@ -10,26 +10,24 @@ of the pytest suite):
 """
 import os
 import sys
-import tempfile
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, ROOT)
+import emul_lib as E
 import validate_lib as VL
-import viewpoint_lib as VP
 from mortal_b200 import dataset_codec as DC
 from viewpoint_lib import hidden_seats, viewpoint
 
-so = os.path.join(tempfile.mkdtemp(), "libmjx_emul_viewpoint_asan.so")
-VP.emul_lib(VP.build_emul(so, extra=("-fsanitize=address,undefined", "-fno-omit-frame-pointer")))  # the sanitised build
+E.lib(sanitize=True)
 rng = np.random.default_rng(43)
 games = VL.emul_games(6, 1, seed0=8100) + VL.emul_games(6, 0, seed0=8200)
 
 
 def scan(jobs):
-    rep = VP.EmulViewReplay(jobs)
+    rep = E.EmulReplay(jobs)
     m = rep.viewpoints()
     rep.close()
     return m
@@ -38,7 +36,7 @@ def scan(jobs):
 # 1. whole single-viewpoint replays with observations, and the all-`?` / odd-`?` logs
 for L in games[:4]:
     vs = [viewpoint(L, p) for p in range(4)]
-    rep = VP.EmulViewReplay(DC.build_jobs(vs, [[p] for p in range(4)]))
+    rep = E.EmulReplay(DC.build_jobs(vs, [[p] for p in range(4)]))
     assert rep.viewpoints().tolist() == [hidden_seats(v) for v in vs]
     for it in range(5000):
         rep.replay_step()

@@ -4,8 +4,6 @@ from the json events), and the host path's per-log expectation."""
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
@@ -13,37 +11,17 @@ import emul_lib as E
 from mortal_b200 import dataset_codec
 from mortal_b200.stat import Stat, _read_counters
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EMUL_SRC = os.path.join(ROOT, "tests", "host_emul", "emul_stat.cc")
-EMUL_SO = os.path.join(ROOT, "tests", "host_emul", "libmjx_emul_stat.so")
 NAMES = _read_counters()  # include/mjx.h MJX_STAT_COUNTERS
 STATUS = {0: "ok", 1: "not start_game", 2: "no deltas", 3: "capacity"}  # include/mjx.h mjx_stat_status
-_emul = None
 
 
-def build_emul(so=EMUL_SO, extra=()):
-    deps = [EMUL_SRC, os.path.join(ROOT, "include", "mjx.h")] + [os.path.join(E.CSRC, f) for f in
-                                                                   ("mjx_stat.cuh", "mjx_mjai.cuh", "mjx_types.cuh", "mjx_port.cuh")]
-    if extra or not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
-        subprocess.check_call(["g++", "-O2" if not extra else "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-DMJX_HOST_EMUL",
-                               "-Wall", "-I" + E.CSRC, "-Wno-unknown-pragmas", *extra, "-o", so, EMUL_SRC])
-    return so
-
-
-def build():
-    build_emul()
-
-
-def emul_lib(path=None):
-    """the emulated kernel; `path` loads another build of emul_stat.cc (the sanitizer run's)"""
-    global _emul
-    if _emul is None or path is not None:
-        L = C.CDLL(path or build_emul())
-        L.emuls_stat_logs.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong,
-                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.emuls_line_deltas.argtypes = [C.c_char_p, C.c_longlong, C.c_void_p]
-        _emul = L
-    return _emul
+def emul_lib():
+    """emul_lib.lib() with the emulated kernel's entries declared"""
+    L = E.lib()
+    L.emuls_stat_logs.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong,
+                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.emuls_line_deltas.argtypes = [C.c_char_p, C.c_longlong, C.c_void_p]
+    return L
 
 
 def encode_deltas(events):

@@ -10,7 +10,8 @@ import pytest
 
 import oracle_lib as O
 import validate_lib as VL
-from viewpoint_lib import EmulViewReplay, hidden_seats, named, viewpoint
+from emul_lib import EmulReplay
+from viewpoint_lib import hidden_seats, named, viewpoint
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ERR_HIDDEN_OWN_TILE = 13
@@ -33,7 +34,7 @@ def _replay(games, players, *, view, obs=None, kan=True):
     from mortal_b200 import dataset_codec as DC
 
     jobs = DC.build_jobs(games, players)
-    rep = EmulViewReplay(jobs, always_include_kan_select=kan)
+    rep = EmulReplay(jobs, always_include_kan_select=kan)
     scan = rep.viewpoints() if view else None
     per = [dict(actions=[], masks=[], meta=[], obs=[]) for _ in range(rep.n_tables)]
     for _ in range(10000):
@@ -152,13 +153,13 @@ def test_scan_edge_cases(logs):
     all_q = [{**ev, "tehais": [["?"] * 13] * 4} if ev["type"] == "start_kyoku" else ev for ev in viewpoint(L, 0)]
     games = [[], v[:1], v[:2], v[:3], v[ky[0]:ky[0] + 1], odd, all_q]
     a = _jobs(games, [[0]] * len(games))
-    rep = EmulViewReplay(a)
+    rep = EmulReplay(a)
     scan = rep.viewpoints()
     rep.close()
     assert scan.tolist() == [hidden_seats(g) for g in games] == [0, 0, 0xE, 0xE, 0xE, 0, 0xF]
     # a job with more start_kyoku words than payloads left is not marked (-1)
     short = dict(a, kyoku=a["kyoku"][: 19 * int(a["ky_off"][4])])
-    rep = EmulViewReplay(short)
+    rep = EmulReplay(short)
     scan = rep.viewpoints()
     rep.close()
     assert scan.tolist() == [0, 0, 0xE, 0xE, -1, -1, -1]

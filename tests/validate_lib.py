@@ -1,12 +1,10 @@
-"""Helpers of the log-validation tests — TEST INFRASTRUCTURE: the emulated validator (tests/host_emul/emul_validate.cc, a
-single-lane host build of csrc/mjx_validate.cuh) and the oracle's restatement of bin/validate_logs.rs (oracle/validate.cc,
-built with the other oracle sources into oracle/libvalidate.so), over the same encoded logs."""
+"""Helpers of the log-validation tests — TEST INFRASTRUCTURE: the emulated validator (emulv_validate_logs of
+tests/host_emul/emul.cc, a single-lane host build of csrc/mjx_validate.cuh) and the oracle's restatement of bin/validate_logs.rs
+(oracle/validate.cc, part of oracle/liboracle.so), over the same encoded logs."""
 from __future__ import annotations
 
 import ctypes as C
 import json
-import os
-import subprocess
 
 import numpy as np
 
@@ -15,68 +13,21 @@ import oracle_lib as O
 from mortal_b200 import mjai_log
 from mortal_b200.validate_logs import REASONS, STATUSES, EncodedLog, Verdict, encode_log, pack, to_verdict
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-ORACLE_DIR = os.path.join(ROOT, "oracle")
-ORACLE_SO = os.path.join(ORACLE_DIR, "libvalidate.so")
-ORACLE_SRCS = [os.path.join(ORACLE_DIR, f) for f in ("algo.cc", "state.cc", "board.cc", "obs.cc", "sp.cc", "validate.cc")]
-EMUL_SRC = os.path.join(ROOT, "tests", "host_emul", "emul_validate.cc")
-EMUL_SO = os.path.join(ROOT, "tests", "host_emul", "libmjx_emul_validate.so")
-_oracle = _emul_lib = None
-
-
-def _stale(target, deps):
-    return not os.path.exists(target) or any(os.path.getmtime(d) > os.path.getmtime(target) for d in deps)
-
-
-def build_oracle(so=ORACLE_SO):
-    deps = ORACLE_SRCS + [os.path.join(ORACLE_DIR, f) for f in os.listdir(ORACLE_DIR) if f.endswith(".h")] + \
-        [os.path.join(ROOT, "include", "mjx.h")]
-    if _stale(so, deps):  # the flags of oracle/Makefile
-        subprocess.check_call(["g++", "-O2", "-g", "-std=c++17", "-fPIC", "-Wall", "-Wextra", "-Wno-unused-parameter", "-ffp-contract=off",
-                               "-pthread", "-shared", "-Wl,--no-undefined", "-o", so, *ORACLE_SRCS])
-    return so
-
-
-def build_emul(so=EMUL_SO, extra=()):
-    deps = [EMUL_SRC, os.path.join(ROOT, "include", "mjx.h")] + [os.path.join(E.CSRC, f) for f in os.listdir(E.CSRC)
-                                                                 if f.endswith((".cuh", ".h"))]
-    if extra or _stale(so, deps):
-        subprocess.check_call(["g++", "-O2" if not extra else "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-DMJX_HOST_EMUL",
-                               "-ffp-contract=off", "-I" + E.CSRC, "-Wno-unknown-pragmas", *extra, "-o", so, EMUL_SRC])
-    return so
-
-
-def build():
-    build_oracle()
-    build_emul()
-
 
 def oracle_lib():
-    global _oracle
-    if _oracle is None:
-        L = C.CDLL(build_oracle())
-        L.orcv_last_error.restype = C.c_char_p
-        L.orcv_init.argtypes = [C.c_char_p]
-        L.orcv_validate_log.argtypes = [C.POINTER(O.OrcEvent), C.c_int, C.POINTER(C.c_int32)]
-        if L.orcv_init(O.DATA_DIR.encode()) != 0:
-            raise RuntimeError(L.orcv_last_error().decode())
-        _oracle = L
-    return _oracle
+    """oracle_lib.lib() with the validator's entries declared"""
+    L = O.lib()
+    L.orcv_last_error.restype = C.c_char_p
+    L.orcv_validate_log.argtypes = [C.POINTER(O.OrcEvent), C.c_int, C.POINTER(C.c_int32)]
+    return L
 
 
-def emul_lib(path=None):
-    """the emulated validator; `path` loads another build of emul_validate.cc (the sanitizer run's)"""
-    global _emul_lib
-    if _emul_lib is None or path is not None:
-        L = C.CDLL(path or build_emul())
-        L.emulv_last_error.restype = C.c_char_p
-        L.emulv_init.argtypes = [C.c_char_p]
-        L.emulv_validate_logs.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p,
-                                          C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]
-        if L.emulv_init(E.DATA_DIR.encode()) != 0:
-            raise RuntimeError(L.emulv_last_error().decode())
-        _emul_lib = L
-    return _emul_lib
+def emul_lib():
+    """emul_lib.lib() with the emulated validator's entry declared"""
+    L = E.lib()
+    L.emulv_validate_logs.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p,
+                                      C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]
+    return L
 
 
 def oracle_events(events):
