@@ -33,10 +33,10 @@ from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
-from . import _logio, dataset_codec
+from . import _cdecl, _logio, dataset_codec
 from .env import ReplayEnv
 
-_ERR_HIDDEN_OWN_TILE = 13  # include/mjx.h MJX_REPLAY_ERR_HIDDEN_OWN_TILE
+_ERR_HIDDEN_OWN_TILE = _cdecl.defines(_cdecl.header())["MJX_REPLAY_ERR_HIDDEN_OWN_TILE"]
 
 
 class Grp:

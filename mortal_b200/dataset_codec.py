@@ -6,6 +6,7 @@ import json
 
 import numpy as np
 
+from . import _cdecl
 from .mjai_log import (ANKAN, CHI, DAHAI, DAIMINKAN, DORA, END_KYOKU, HORA, KAKAN, PON, REACH, REACH_ACCEPTED, RYUKYOKU,
                        START_KYOKU, TILE_NAMES, TSUMO)
 
@@ -24,7 +25,7 @@ def _word(ty, actor=0, target=0, pai=37, tsumogiri=0, c=(0, 0, 0, 0)):
 KYOKU_WORDS = 19  # csrc/mjx_replay.cuh REPLAY_KYOKU_WORDS: 2 score words + the 136-byte wall (17 words)
 
 
-HORA_WORDS = 2  # include/mjx.h MJX_HORA_WORDS
+HORA_WORDS = _cdecl.defines(_cdecl.header())["MJX_HORA_WORDS"]
 
 
 def _hora_entry(ev, t):

@@ -20,7 +20,6 @@ import gzip
 import json
 import math
 import os
-import re
 import sys
 from concurrent.futures import ThreadPoolExecutor
 
@@ -299,13 +298,9 @@ def _host_log_stat(path: str, player_name: str) -> Stat:
 def _read_counters():
     """the counter names of include/mjx.h MJX_STAT_COUNTERS, in the order k_stat_logs writes them (the header is their single
     definition)"""
-    from . import _lib
+    from . import _cdecl
 
-    with open(os.path.join(os.path.dirname(_lib.HERE), "include", "mjx.h")) as f:
-        text = f.read()
-    block = text[text.index("#define MJX_STAT_COUNTERS(X)"):]
-    block = block[:block.index("#define MJX_STAT_ENUM_")]
-    return tuple(re.findall(r"X\((\w+)\)", block))
+    return tuple(name for (name,) in _cdecl.xmacro(_cdecl.header(), "MJX_STAT_COUNTERS"))
 
 
 def _seat_mask(blob: bytes, b: int, e: int, player_name: str):

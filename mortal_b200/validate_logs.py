@@ -15,30 +15,20 @@ import glob
 import gzip
 import json
 import os
-import re
 import sys
 from concurrent.futures import ThreadPoolExecutor
 from dataclasses import dataclass
 
 import numpy as np
 
-from . import _lib
+from . import _cdecl, _lib
 from .dataset_codec import HORA_WORDS, KYOKU_WORDS, check_event, encode_events
 
-STATUSES = ("OK", "CHECK", "UPDATE", "PARSE", "UNSUPPORTED")  # include/mjx.h mjx_verdict_status
+# indexed by code, read from include/mjx.h (their single definition): the verdict status names (mjx_verdict_status, whose codes
+# run 0, 1, ...) and the reason names (MJX_VALIDATE_REASONS)
+STATUSES = tuple(name.removeprefix("MJX_V_") for name in _cdecl.enum(_cdecl.header(), "mjx_verdict_status"))
+REASONS = tuple(name for _, name in _cdecl.xmacro(_cdecl.header(), "MJX_VALIDATE_REASONS"))
 CHUNK_LOGS = 4096  # logs decoded and validated per launch by the CLI: bounds its memory whatever the corpus size
-
-
-def _read_reasons():
-    """the reason names of include/mjx.h MJX_VALIDATE_REASONS, indexed by code (the header is their single definition)"""
-    with open(os.path.join(os.path.dirname(_lib.HERE), "include", "mjx.h")) as f:
-        text = f.read()
-    block = text[text.index("#define MJX_VALIDATE_REASONS(X)"):]
-    block = block[:block.index("#define MJX_REASON_ENUM_")]
-    return tuple(name for _, name in re.findall(r'X\((\w+), "([^"]*)"\)', block))
-
-
-REASONS = _read_reasons()
 
 
 @dataclass(frozen=True)

@@ -94,13 +94,14 @@ assert v == [None] * n_logs
 print(f"end to end: {dt:.2f} s = {n_logs / dt:.0f} logs/s")
 
 # the oracle restatement on all host threads (the ctypes call releases the GIL); JSON decoding outside the timed window
+import oracle_lib as O
 import validate_lib as VL
 
 sub = []
 for t in texts[: args.cpu_logs]:
     evs = [json.loads(x) for x in t.splitlines() if x.strip()]
     sub.append((VL.oracle_events(evs), len(evs)))
-VL.oracle_lib()
+O.lib()
 cores = len(os.sched_getaffinity(0))
 t0 = time.perf_counter()
 with cf.ThreadPoolExecutor(cores) as ex:

@@ -1,6 +1,6 @@
 """Builds and binds tests/host_emul/libmjx_emul.so — TEST INFRASTRUCTURE: every tests/host_emul/*.cc (single-lane host builds
-of the product's device sources, -DMJX_HOST_EMUL) linked into one library. This module binds emul.cc's entries; the feature
-helpers (validate_lib, mjai_lib, ...) declare their own entries on lib(). Never used by mortal_b200/."""
+of the product's device sources, -DMJX_HOST_EMUL) linked into one library, with every entry of their extern "C" blocks bound
+from its C definition. Never used by mortal_b200/."""
 import ctypes as C
 import glob
 import os
@@ -8,6 +8,8 @@ import subprocess
 import tempfile
 
 import numpy as np
+
+from mortal_b200 import _cdecl
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HOST_EMUL = os.path.join(ROOT, "tests", "host_emul")
@@ -37,45 +39,18 @@ def build(sanitize=False):
     return so
 
 
+def _entries():
+    """the ctypes signatures of every extern "C" function of tests/host_emul/*.cc"""
+    srcs = sorted(glob.glob(os.path.join(HOST_EMUL, "*.cc")))
+    return _cdecl.functions("".join(open(s).read() for s in srcs), "emul")
+
+
 def lib(sanitize=False):
-    """The library, loaded once, with emul.cc's entries bound and the lookup tables loaded. A sanitizer run calls
-    lib(sanitize=True) before anything else loads the library."""
+    """The library, loaded once, with every entry bound and the lookup tables loaded. A sanitizer run calls lib(sanitize=True)
+    before anything else loads the library."""
     global _lib
     if _lib is None:
-        L = C.CDLL(build(sanitize))
-        L.emul_last_error.restype = C.c_char_p
-        L.emul_init.argtypes = [C.c_char_p]
-        L.emul_shanten.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
-        L.emul_make_wall.argtypes = [C.c_uint64, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_void_p]
-        L.emul_run.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
-                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_int64, C.c_int]
-        L.emul_env_create.restype = C.c_void_p
-        L.emul_env_create.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
-        L.emul_env_destroy.argtypes = [C.c_void_p]
-        L.emul_env_step.argtypes = [C.c_void_p, C.c_void_p]
-        L.emul_env_num_rows.argtypes = [C.c_void_p]
-        L.emul_env_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.emul_env_policy_test.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-        L.emul_env_encode_obs.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-        L.emul_env_encode_obs_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
-        L.emul_sp_overflows.restype = C.c_long
-        L.emul_replay_create.restype = C.c_void_p
-        L.emul_replay_create.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int]
-        L.emul_replay_step.argtypes = [C.c_void_p]
-        L.emul_replay_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        L.emul_env_errs.argtypes = [C.c_void_p, C.c_void_p]
-        L.emul_env_row_steps.argtypes = [C.c_void_p, C.c_void_p]
-        L.emul_env_set_quick_eval.argtypes = [C.c_void_p, C.c_void_p]
-        L.emul_env_enable_grp.argtypes = [C.c_void_p, C.c_int]
-        L.emul_env_read_grp.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        L.emul_env_encode_invisible.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-        L.emul_replay_trust_seeds.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
-        L.emul_replay_encode_invisible.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-        L.emul_env_enable_log.argtypes = [C.c_void_p, C.c_int]
-        L.emul_env_read_log.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        L.emul_env_log_lens.argtypes = [C.c_void_p, C.c_void_p]
-        L.emul_env_results.argtypes = [C.c_void_p] + [C.c_void_p] * 5
-        L.emul_replay_viewpoints.argtypes = [C.c_void_p, C.c_void_p]
+        L = _cdecl.bind(C.CDLL(build(sanitize)), _entries())
         if L.emul_init(DATA_DIR.encode()) != 0:
             raise RuntimeError(L.emul_last_error().decode())
         _lib = L
@@ -88,7 +63,7 @@ def pylib():
     """lib()'s file loaded again with ctypes.PyDLL, whose calls hold the GIL: for entries that call back into Python"""
     global _pylib
     if _pylib is None:
-        _pylib = C.PyDLL(lib()._name)
+        _pylib = _cdecl.bind(C.PyDLL(lib()._name), _entries())
     return _pylib
 
 

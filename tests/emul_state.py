@@ -10,14 +10,7 @@ from mortal_b200.libriichi.state import PlayerView
 
 class EmulStateBackend:
     def __init__(self):
-        L = self.L = E.lib()
-        L.emul_state_create.restype = C.c_void_p
-        L.emul_state_create.argtypes = [C.c_int, C.c_void_p]
-        L.emul_state_update.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.emul_state_view.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-        L.emul_state_rows.argtypes = [C.c_void_p, C.c_void_p]
-        L.emul_state_query.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
-        L.emul_state_copy.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
+        self.L = E.lib()
 
     def create(self, player_ids, version=4):
         ids = np.ascontiguousarray(player_ids, dtype=np.uint8)

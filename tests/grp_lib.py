@@ -2,44 +2,21 @@
 k_grp_logs reads (stat_lib.encode: the decoder's layout, encoded on the host), and the host path's per-log expectation."""
 from __future__ import annotations
 
-import ctypes as C
-import os
-import re
-
 import numpy as np
 
 import emul_lib as E
 import stat_lib as S
+from mortal_b200 import _cdecl
 from mortal_b200.dataset import Grp
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _statuses():
-    """include/mjx.h mjx_grp_status: code -> name"""
-    with open(os.path.join(ROOT, "include", "mjx.h")) as f:
-        text = f.read()
-    block = text[text.index("enum mjx_grp_status"):]
-    block = block[:block.index("}")]
-    return {int(v): k for k, v in re.findall(r"MJX_GRP_(\w+) = (\d+)", block)}
-
-
-STATUS = _statuses()
+STATUS = {v: k.removeprefix("MJX_GRP_") for k, v in _cdecl.enum(_cdecl.header(), "mjx_grp_status").items()}  # code -> name
 encode = S.encode
-
-
-def emul_lib():
-    """emul_lib.lib() with the emulated kernel's entry declared"""
-    L = E.lib()
-    L.emulg_grp_logs.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong,
-                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    return L
 
 
 def run_emul(a, n_hdr=None, n_kyoku_words=None):
     """the emulated kernel over encode()'s arrays -> (feat int32 [n_kyoku, 7], rank uint8 [n, 4], final int64 [n, 4], status int32 [n]);
     n_hdr / n_kyoku_words override the capacities (hostile-array tests)"""
-    L = emul_lib()
+    L = E.lib()
     n = len(a["ev_off"])
     nk = len(a["kyoku"]) if n_kyoku_words is None else n_kyoku_words
     feat = np.full((max(nk // 19, 1), 7), -1, dtype=np.int32)

@@ -4,7 +4,6 @@ through pad_sequence + pack_padded_sequence (collate), GRP.forward_packed, get_l
 GrpFileDatasetsIter over stub or real file lists."""
 from __future__ import annotations
 
-import ctypes as C
 import random
 
 import numpy as np
@@ -14,18 +13,6 @@ from torch.nn.utils.rnn import pack_padded_sequence, pad_sequence
 
 import emul_lib as E
 from reward_lib import RefGRP, random_feature, random_grp  # noqa: F401  (re-exported for the tests)
-
-
-def emul_lib():
-    """emul_lib.lib() with the emulated kernels' entries declared"""
-    L = E.lib()
-    L.emult_grp_train.restype = C.c_int
-    L.emult_grp_train.argtypes = ([C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_int, C.c_int,
-                                   C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 5 + [C.c_int]
-                                  + [C.c_void_p] * 5 + [C.c_longlong])
-    L.emult_scratch_bytes.restype = C.c_longlong
-    L.emult_scratch_bytes.argtypes = [C.c_int] * 5
-    return L
 
 
 def pack(grp):
@@ -51,7 +38,7 @@ def run_emul(weights, hidden, layers, feats, game, length, rank, grad=True, jobs
     """emult_grp_train -> (rc, loss, acc, grad [n_weights] (NaN-filled when not written), status [B]). feats: per-game [L, 7]
     arrays or a dict with the packed `feat` and `game_off` (hostile runs); jobs: override of jobs_of(game, length); the other
     keywords override the counts passed"""
-    L = emul_lib()
+    L = E.lib()
     if isinstance(feats, dict):
         feat, off = np.ascontiguousarray(feats["feat"], dtype=np.float64), np.ascontiguousarray(feats["game_off"], dtype=np.int32)
     else:

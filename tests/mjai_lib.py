@@ -3,7 +3,6 @@ the host path's arrays for comparison, and two seeded corpora: format variations
 text, and byte-level hostile mutations."""
 from __future__ import annotations
 
-import ctypes as C
 import json
 import os
 
@@ -16,18 +15,10 @@ from mortal_b200.validate_logs import EncodedLog, encode_log
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def emul_lib():
-    """emul_lib.lib() with the emulated decoder's entry declared"""
-    L = E.lib()
-    L.emulm_decode.argtypes = [C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
-                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong]
-    return L
-
-
 def emul_decode(blobs, augment=False):
     """bytes per log -> per log None (declined) or dict(hdr, kyoku [k, 19], hora [h, 2], lines, first = bytes of the first event
     line), through the count and fill calls of the emulated decoder"""
-    L = emul_lib()
+    L = E.lib()
     n = len(blobs)
     buf = np.frombuffer(b"".join(blobs) or b"\0", dtype=np.uint8)
     off = np.zeros(n + 1, dtype=np.int64)

@@ -9,38 +9,12 @@ import numpy as np
 import emul_lib as E
 
 
-def emul_lib():
-    """emul_lib.lib() with the emulated writer's entries declared"""
-    L = E.lib()
-    L.emulw_format_f32.restype = C.c_longlong
-    L.emulw_format_f32.argtypes = [C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong]
-    L.emulw_render.restype = C.c_int
-    L.emulw_render.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
-                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                               C.c_longlong]
-    L.emulw_meta_record.restype = C.c_int
-    L.emulw_meta_record.argtypes = ([C.c_longlong] + [C.c_void_p] * 4 + [C.c_int, C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_int]
-                                    + [C.c_void_p] * 7 + [C.c_longlong, C.c_longlong])
-    return L
-
-
-def callback_lib():
-    """emul_lib.pylib() with the formatter's comparison entries declared: they call back into this interpreter
-    (PyOS_double_to_string) and need the GIL held"""
-    L = E.pylib()
-    L.emulw_sweep.restype = C.c_longlong
-    L.emulw_sweep.argtypes = [C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
-    L.emulw_check.restype = C.c_longlong
-    L.emulw_check.argtypes = [C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
-    return L
-
-
 def format_f32(values) -> list[str]:
     """the emulated formatter over float32 values (or uint32 bit patterns)"""
     bits = np.ascontiguousarray(np.asarray(values).view(np.uint32) if np.asarray(values).dtype == np.float32 else values,
                                 dtype=np.uint32)
     out = np.zeros(32 * len(bits) + 1, dtype=np.uint8)
-    n = emul_lib().emulw_format_f32(bits.ctypes.data, len(bits), out.ctypes.data, out.size)
+    n = E.lib().emulw_format_f32(bits.ctypes.data, len(bits), out.ctypes.data, out.size)
     assert n >= 0
     return out[:n].tobytes().decode("ascii").split("\n")[:-1]
 
@@ -52,7 +26,7 @@ def _py_fns():
 def sweep(lo: int, hi: int, step: int = 1):
     """(mismatches, first mismatching bit pattern) of the formatter against PyOS_double_to_string over [lo, hi)"""
     first = C.c_uint64(0)
-    n = callback_lib().emulw_sweep(lo, hi, step, *_py_fns(), C.byref(first))
+    n = E.pylib().emulw_sweep(lo, hi, step, *_py_fns(), C.byref(first))
     return int(n), int(first.value)
 
 
@@ -60,7 +34,7 @@ def check(bits):
     """(mismatches, first mismatching bit pattern) of the formatter against PyOS_double_to_string over a list of patterns"""
     bits = np.ascontiguousarray(bits, dtype=np.uint32)
     first = C.c_uint64(0)
-    n = callback_lib().emulw_check(bits.ctypes.data, len(bits), *_py_fns(), C.byref(first))
+    n = E.pylib().emulw_check(bits.ctypes.data, len(bits), *_py_fns(), C.byref(first))
     return int(n), int(first.value)
 
 
@@ -68,7 +42,7 @@ def render(words, lens, bounds=None, recs=None):
     """the emulated count + fill over host arrays: (status int32 [n_games], list of text bytes per game (None: non-zero status))"""
     from mortal_b200 import mjai_write
 
-    L = emul_lib()
+    L = E.lib()
     words = np.ascontiguousarray(words, dtype=np.uint64)
     lens = np.ascontiguousarray(lens, dtype=np.int32)
     n, cap = words.shape
@@ -90,7 +64,7 @@ class EmulRecords:
     """DeviceMetaRecorder's record arrays on the host, appended by the host build of k_meta_record (emulw_meta_record)"""
 
     def __init__(self, cap):
-        self.L = emul_lib()
+        self.L = E.lib()
         self.cap, self.count, self.calls, self.max_cycle = cap, 0, [], -1
         self.table, self.cycle = np.zeros(cap, np.int32), np.zeros(cap, np.int32)
         self.seat, self.info = np.zeros(cap, np.uint8), np.zeros((cap, 4), np.int32)

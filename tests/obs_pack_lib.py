@@ -2,7 +2,6 @@
 (tests/host_emul/emul_obs_pack.cc) and observation fixtures of every version from the oracle."""
 from __future__ import annotations
 
-import ctypes as C
 import os
 
 import numpy as np
@@ -14,27 +13,13 @@ ROWS = {(1, False): 938, (2, False): 942, (3, False): 934, (4, False): 1012, (1,
         (4, True): 217}
 
 
-def emul_lib():
-    """emul_lib.lib() with the emulated codec's entries declared"""
-    L = E.lib()
-    L.emulp_record_bytes.restype = C.c_int
-    L.emulp_record_bytes.argtypes = [C.c_int, C.c_int]
-    L.emulp_pack.restype = C.c_int
-    L.emulp_pack.argtypes = [C.c_int, C.c_int, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p]
-    L.emulp_unpack.restype = C.c_int
-    L.emulp_unpack.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p]
-    L.emulp_value_rows.restype = C.c_int
-    L.emulp_value_rows.argtypes = [C.c_int, C.c_int, C.c_void_p]
-    return L
-
-
 def record_bytes(version, invisible):
-    return emul_lib().emulp_record_bytes(version, int(invisible))
+    return E.lib().emulp_record_bytes(version, int(invisible))
 
 
 def value_rows(version, invisible):
     buf = np.zeros(96, dtype=np.int16)
-    n = emul_lib().emulp_value_rows(version, int(invisible), buf.ctypes.data)
+    n = E.lib().emulp_value_rows(version, int(invisible), buf.ctypes.data)
     assert n >= 0
     return buf[:n].astype(np.int64)
 
@@ -48,8 +33,8 @@ def pack(x, version, invisible, pitch=None, n=None):
     rb = max(record_bytes(version, invisible), 0)
     rec = np.full((max(n, 0), rb), 0xA5, dtype=np.uint8)
     status = np.full(max(n, 0), -7, dtype=np.int32)
-    rc = emul_lib().emulp_pack(version, int(invisible), n, x.ctypes.data if x.size else None, pitch, rec.ctypes.data if rec.size else None,
-                               status.ctypes.data if n > 0 else None)
+    rc = E.lib().emulp_pack(version, int(invisible), n, x.ctypes.data if x.size else None, pitch, rec.ctypes.data if rec.size else None,
+                            status.ctypes.data if n > 0 else None)
     return rc, rec, status
 
 
@@ -58,8 +43,8 @@ def unpack(rec, idx, version, invisible, n_records=None):
     rec = np.ascontiguousarray(rec, dtype=np.uint8)
     idx = np.ascontiguousarray(idx, dtype=np.int64)
     out = np.full((len(idx), ROWS.get((version, bool(invisible)), 938), 34), np.nan, dtype=np.float32)
-    rc = emul_lib().emulp_unpack(version, int(invisible), rec.ctypes.data if rec.size else None, len(rec) if n_records is None else n_records,
-                                 idx.ctypes.data if idx.size else None, len(idx), out.ctypes.data if out.size else None)
+    rc = E.lib().emulp_unpack(version, int(invisible), rec.ctypes.data if rec.size else None, len(rec) if n_records is None else n_records,
+                              idx.ctypes.data if idx.size else None, len(idx), out.ctypes.data if out.size else None)
     return rc, out
 
 

@@ -1,4 +1,5 @@
-"""ctypes binding of oracle/liboracle.so — TEST INFRASTRUCTURE (never imported by mortal_b200/)."""
+"""ctypes binding of oracle/liboracle.so, every entry of oracle/capi.cc and oracle/validate.cc bound from its C definition —
+TEST INFRASTRUCTURE (never imported by mortal_b200/)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -7,6 +8,8 @@ import os
 import subprocess
 
 import numpy as np
+
+from mortal_b200 import _cdecl
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ORACLE_DIR = os.path.join(ROOT, "oracle")
@@ -146,75 +149,8 @@ def lib():
     global _lib
     if _lib is not None:
         return _lib
-    L = C.CDLL(build())
-    L.orc_last_error.restype = C.c_char_p
-    L.orc_init.argtypes = [C.c_char_p]
-    L.orc_shanten.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
-    L.orc_agari.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
-    L.orc_point.argtypes = [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int32)]
-    L.orc_check_ankan_after_riichi.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
-    L.orc_rankings.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-    L.orc_agari_key.argtypes = [C.c_void_p, C.c_void_p]
-    L.orc_agari_key.restype = C.c_uint32
-    L.orc_agari_lookup.argtypes = [C.c_uint32, C.c_void_p]
-    L.orc_make_wall.argtypes = [C.c_uint64, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_void_p]
-    L.orc_sha3_256.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    L.orc_chacha12.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-    L.orc_ps_new.restype = C.c_void_p
-    L.orc_ps_new.argtypes = [C.c_int]
-    L.orc_ps_free.argtypes = [C.c_void_p]
-    L.orc_ps_clone.restype = C.c_void_p
-    L.orc_ps_clone.argtypes = [C.c_void_p]
-    L.orc_ps_update.restype = C.c_int64
-    L.orc_ps_update.argtypes = [C.c_void_p, C.POINTER(OrcEvent)]
-    L.orc_ps_validate_reaction.argtypes = [C.c_void_p, C.POINTER(OrcEvent)]
-    L.orc_ps_view_get.argtypes = [C.c_void_p, C.POINTER(PsView)]
-    L.orc_ps_set_tehai.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-    L.orc_ps_update_waits_and_furiten.argtypes = [C.c_void_p]
-    L.orc_ps_set_can_chi_from_tile.argtypes = [C.c_void_p, C.c_int]
-    L.orc_ps_set_can_chi_from_tile.restype = C.c_uint32
-    L.orc_ps_get_rank.argtypes = [C.c_int, C.c_void_p]
-    L.orc_ps_agari_points.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_int32)]
-    L.orc_ps_rule_based_agari.argtypes = [C.c_void_p]
-    L.orc_ps_rule_based_agari_slow.argtypes = [C.c_void_p, C.c_int, C.c_int]
-    L.orc_ps_discard_candidates.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    L.orc_obs_rows.argtypes = [C.c_int]
-    L.orc_ps_encode_obs.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
-    L.orc_ps_legal_mask.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-    L.orc_sp_calc.argtypes = [C.POINTER(SpIn), C.POINTER(SpCand), C.c_int]
-    L.orc_game_new.restype = C.c_void_p
-    L.orc_game_new.argtypes = [C.c_uint64, C.c_uint64, C.c_int, C.c_int]
-    L.orc_game_free.argtypes = [C.c_void_p]
-    L.orc_game_poll.argtypes = [C.c_void_p]
-    L.orc_game_state.restype = C.c_void_p
-    L.orc_game_state.argtypes = [C.c_void_p, C.c_int]
-    L.orc_game_set_reaction.argtypes = [C.c_void_p, C.c_int, C.POINTER(OrcEvent)]
-    L.orc_game_set_action.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
-    L.orc_game_advance_step.argtypes = [C.c_void_p]
-    L.orc_game_finish.argtypes = [C.c_void_p, C.c_void_p]
-    L.orc_game_info.argtypes = [C.c_void_p, C.c_void_p]
-    L.orc_game_log.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-    L.orc_gameplay_load.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 7
-    L.orc_gameplay_load_oracle.argtypes = ([C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 7
-                                           + [C.c_uint64, C.c_uint64, C.c_int, C.c_void_p, C.c_void_p])
-    L.orc_run_batch.argtypes = [C.POINTER(RunCfg), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.POINTER(RunOut)]
-    L.orc_run_replay.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_void_p,
-                                 C.c_void_p, C.c_void_p]
-    L.orc_run_replay2.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
-                                  C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.orc_run_replay3.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
-                                  C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.orc_run_sample_obs.argtypes = [C.POINTER(RunCfg), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                     C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.orc_oracle_obs_rows.argtypes = [C.c_int]
-    L.orc_game_encode_oracle_obs.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
-    L.orc_batch_new.restype = C.c_void_p
-    L.orc_batch_new.argtypes = [C.POINTER(RunCfg), C.c_void_p, C.c_void_p]
-    L.orc_batch_free.argtypes = [C.c_void_p]
-    L.orc_batch_run.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.POINTER(RunOut)]
-    L.orc_policy_hash.restype = C.c_uint64
-    L.orc_policy_hash.argtypes = [C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint32]
+    srcs = [os.path.join(ORACLE_DIR, f) for f in ("capi.cc", "validate.cc")]
+    L = _cdecl.bind(C.CDLL(build()), _cdecl.functions("".join(open(s).read() for s in srcs), "orc"))
     if L.orc_init(DATA_DIR.encode()) != 0:
         raise RuntimeError(L.orc_last_error().decode())
     _lib = L

@@ -4,7 +4,6 @@ with the literal prefix-list formulation (pack_padded_sequence over feature[:k+1
 dataloader.py populate_buffer."""
 from __future__ import annotations
 
-import ctypes as C
 from itertools import permutations
 
 import numpy as np
@@ -13,16 +12,6 @@ from torch import nn
 from torch.nn.utils.rnn import pack_padded_sequence, pad_sequence
 
 import emul_lib as E
-
-
-def emul_lib():
-    """emul_lib.lib() with the emulated kernels' entry declared"""
-    L = E.lib()
-    L.emulr_grp_reward.restype = C.c_int
-    L.emulr_grp_reward.argtypes = ([C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_int, C.c_int,
-                                    C.c_void_p, C.c_int, C.c_void_p, C.c_longlong] + [C.c_void_p] * 8 + [C.c_int]
-                                   + [C.c_void_p] * 4)
-    return L
 
 
 # ---------------------------------------------------------------- the reference, restated
@@ -133,7 +122,7 @@ def run_emul(weights, hidden, layers, feats, jobs=None, pts=(3, 1, -1, -3), unif
     """emulr_grp_reward -> (rc, matrix [R, 4, 4], steps, reward, rank, status). feats: per-game [L, 7] arrays, or a dict with the
     packed `feat` and `game_off` (hostile-array runs); jobs: dict of move_off, job_game, job_player, at_kyoku, apply_gamma, dones,
     rank, final (numpy); n_rows / n_weights override the counts passed"""
-    L = emul_lib()
+    L = E.lib()
     if isinstance(feats, dict):
         feat, off = np.ascontiguousarray(feats["feat"], dtype=np.float64), np.ascontiguousarray(feats["game_off"], dtype=np.int32)
     else:

@@ -3,8 +3,6 @@ a host encoder of the arrays k_stat_logs reads (event words and payloads from da
 from the json events), and the host path's per-log expectation."""
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 
 import emul_lib as E
@@ -13,15 +11,6 @@ from mortal_b200.stat import Stat, _read_counters
 
 NAMES = _read_counters()  # include/mjx.h MJX_STAT_COUNTERS
 STATUS = {0: "ok", 1: "not start_game", 2: "no deltas", 3: "capacity"}  # include/mjx.h mjx_stat_status
-
-
-def emul_lib():
-    """emul_lib.lib() with the emulated kernel's entries declared"""
-    L = E.lib()
-    L.emuls_stat_logs.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong,
-                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.emuls_line_deltas.argtypes = [C.c_char_p, C.c_longlong, C.c_void_p]
-    return L
 
 
 def encode_deltas(events):
@@ -55,7 +44,7 @@ def encode(games):
 def run_emul(a, seats, n_hdr=None, n_kyoku_words=None):
     """the emulated kernel over encode()'s arrays -> (int64 [n, MJX_STAT_N], int32 [n]); n_hdr / n_kyoku_words override the
     capacities (hostile-array tests)"""
-    L = emul_lib()
+    L = E.lib()
     n = len(a["ev_off"])
     seats = np.ascontiguousarray(seats, dtype=np.uint8)
     out = np.full((n, len(NAMES)), -1, dtype=np.int64)
@@ -72,7 +61,7 @@ def run_emul(a, seats, n_hdr=None, n_kyoku_words=None):
 def line_deltas(line: bytes):
     """mjai_line_deltas of the decoder (host build) -> (has_deltas, [4 ints])"""
     d = np.zeros(4, dtype=np.int32)
-    has = emul_lib().emuls_line_deltas(line, len(line), d.ctypes.data)
+    has = E.lib().emuls_line_deltas(line, len(line), d.ctypes.data)
     return bool(has), [int(x) for x in d]
 
 

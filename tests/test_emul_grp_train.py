@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 import torch
 
+import emul_lib as E
 import grp_train_lib as T
 
 LENGTHS = (1, 2, 8, 20, 64)
@@ -83,7 +84,7 @@ def test_argument_checks():
     assert T.run_emul(w, h, nl, f, game, length, rank, n_rows=0)[0] == -2
     assert T.run_emul(w, h, nl, f, game, length, rank, n_samples=0)[0] == -2
     assert T.run_emul(w, h, nl, f, game, length, rank, scratch_bytes=8)[0] == -2
-    L = T.emul_lib()
+    L = E.lib()
     assert L.emult_scratch_bytes(8, 2, 3, 4, 5) == -2  # more jobs than samples
     assert L.emult_scratch_bytes(8, 2, 3, 2, 0) == -2
     assert T.run_emul(*T.pack(T.random_grp(256, 4, 2)), f, game, length, rank)[0] == 0  # the largest shape

@@ -15,16 +15,23 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 def test_c_abi_exports_every_declared_symbol():
     import mortal_b200
-    from mortal_b200 import _lib
+    from mortal_b200 import _cdecl, _lib
 
     L = mortal_b200.load()
-    header = open(os.path.join(ROOT, "include", "mjx.h")).read()
+    header = _cdecl.header()
     declared = set(re.findall(r"\b(mjx_[a-z0-9_]+)\s*\(", header))
     declared -= {"mjx_status"}
-    assert declared, "no declarations parsed"
+    assert len(declared) == 90, "not every declaration parsed"
     for name in declared:
         assert hasattr(L, name), f"libmjx.so does not export {name}"
     assert declared == set(_lib.SYMBOLS), declared ^ set(_lib.SYMBOLS)
+    # every prototype's parameter list, found without the reader: each entry is bound with one argtype per parameter
+    prototypes = dict(re.findall(r"^[\w ]+\*? *(mjx_\w+)\(([^)]*)\)", re.sub(r"/\*.*?\*/", "", header, flags=re.S), re.M))
+    assert set(prototypes) == declared
+    for name, (restype, argtypes) in _lib.SYMBOLS.items():
+        fn = getattr(L, name)
+        assert fn.restype is restype and fn.argtypes == argtypes, name
+        assert len(argtypes) == (0 if prototypes[name] == "void" else prototypes[name].count(",") + 1), name
     assert C.sizeof(_lib.AgariIn) == 62 and C.sizeof(_lib.AgariOut) == 16
 
 

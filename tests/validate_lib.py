@@ -14,22 +14,6 @@ from mortal_b200 import mjai_log
 from mortal_b200.validate_logs import REASONS, STATUSES, EncodedLog, Verdict, encode_log, pack, to_verdict
 
 
-def oracle_lib():
-    """oracle_lib.lib() with the validator's entries declared"""
-    L = O.lib()
-    L.orcv_last_error.restype = C.c_char_p
-    L.orcv_validate_log.argtypes = [C.POINTER(O.OrcEvent), C.c_int, C.POINTER(C.c_int32)]
-    return L
-
-
-def emul_lib():
-    """emul_lib.lib() with the emulated validator's entry declared"""
-    L = E.lib()
-    L.emulv_validate_logs.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p,
-                                      C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]
-    return L
-
-
 def oracle_events(events):
     """mjai dicts -> the oracle's flat events; a hora's `has_deltas` carries the presence of `deltas` (bit 0) and of
     `ura_markers` (bit 1)"""
@@ -43,7 +27,7 @@ def oracle_events(events):
 def oracle_validate_events(arr, n):
     """the oracle's (status, reason, line, seat) codes of one log given as oracle_events()"""
     out = (C.c_int32 * 4)()
-    L = oracle_lib()
+    L = O.lib()
     if L.orcv_validate_log(arr, n, out) != 0:
         raise RuntimeError(L.orcv_last_error().decode())
     return tuple(out)
@@ -53,7 +37,7 @@ def emul_run_packed(p) -> np.ndarray:
     """the emulated mjx_validate_logs over validate_logs.pack()'s arrays -> int32 [n, 4]"""
     n = len(p["ev_off"])
     out = np.zeros((n, 4), dtype=np.int32)
-    rc = emul_lib().emulv_validate_logs(n, p["hdr"].ctypes.data, p["ev_off"].ctypes.data, p["ev_cnt"].ctypes.data, len(p["hdr"]),
+    rc = E.lib().emulv_validate_logs(n, p["hdr"].ctypes.data, p["ev_off"].ctypes.data, p["ev_cnt"].ctypes.data, len(p["hdr"]),
                                      p["kyoku"].ctypes.data, p["ky_off"].ctypes.data, len(p["kyoku"]), p["hora"].ctypes.data,
                                      p["hora_off"].ctypes.data, len(p["hora"]), out.ctypes.data)
     assert rc == 0
