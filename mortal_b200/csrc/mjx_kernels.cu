@@ -14,6 +14,7 @@
 #include "mjx_validate.cuh"
 #include "mjx_mjai.cuh"
 #include "mjx_mjai_write.cuh"
+#include "mjx_selfplay.cuh"
 #include "mjx_stat.cuh"
 #include "mjx_grp.cuh"
 #include "mjx_reward.cuh"
@@ -1164,6 +1165,66 @@ __global__ void __launch_bounds__(MW_WARPS * 32) k_mjai_render(MwView V) {
     }
 }
 
+// ---- arena event words -> replay arrays (csrc/mjx_selfplay.cuh)
+// One game per warp. Lane 0 queues the next 32 event starts, each lane checks and converts one event; the event, payload and hora
+// indices come from the running counts plus ballot prefix counts. The walk and the statuses are warp-uniform. FILL writes the
+// games whose counts say OK, start_game first and end_game after the last event.
+template <bool FILL>
+__global__ void __launch_bounds__(AW_WARPS * 32) k_arena_words(AwView V) {
+    __shared__ int s_start[AW_WARPS][32];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const int g = blockIdx.x * AW_WARPS + wid;
+    if (g >= V.n_games) return;
+    if (FILL && V.counts[4 * g] != MJX_AW_OK) return;
+    const u64* w;
+    int n;
+    int st = aw_game_words(V, g, &w, &n);
+    const long long e0 = FILL ? V.ev_off[g] : 0, k0 = FILL ? V.ky_off[g] : 0, h0 = FILL ? V.hora_off[g] : 0;
+    if (FILL && lane == 0) aw_fill_bound(V, AW_START_GAME, e0, 1);
+    int n_ev = 0, n_ky = 0, n_ho = 0;
+    const unsigned below = (1u << lane) - 1;
+    for (int pos = 0; st == MJX_AW_OK && pos < n;) {
+        int cnt = 0, nx = pos, wst = MJX_AW_OK;
+        if (lane == 0) {
+            while (cnt < 32 && nx < n) {
+                const int t = aw_next(w, n, nx);
+                if (t < 0) { wst = -t; break; }
+                s_start[wid][cnt++] = nx;
+                nx = t;
+            }
+        }
+        __syncwarp();
+        cnt = __shfl_sync(~0u, cnt, 0);
+        nx = __shfl_sync(~0u, nx, 0);
+        wst = __shfl_sync(~0u, wst, 0);
+        const int i = lane < cnt ? s_start[wid][lane] : 0;
+        const int est = lane < cnt ? aw_check(w, i) : MJX_AW_OK;
+        const int ty = lane < cnt ? (int)(w[i] & 0xFF) : 0;
+        const unsigned bad = __ballot_sync(~0u, est != MJX_AW_OK);
+        const unsigned ky = __ballot_sync(~0u, ty == AW_START_KYOKU), ho = __ballot_sync(~0u, ty == AW_HORA);
+        if (FILL && !bad && lane < cnt) {
+            const int e = 1 + n_ev + lane;  // the event's index in the game (start_game is 0)
+            aw_fill_event(V, w, i, e0 + e, e + 1, k0 + n_ky + __popc(ky & below), h0 + n_ho + __popc(ho & below));
+        }
+        n_ev += cnt;
+        n_ky += __popc(ky);
+        n_ho += __popc(ho);
+        __syncwarp();  // s_start is refilled by lane 0
+        st = bad ? MJX_AW_CORRUPT : wst;
+        pos = nx;
+    }
+    if (lane == 0) {
+        if (FILL && st == MJX_AW_OK) aw_fill_bound(V, AW_END_GAME, e0 + n_ev + 1, n_ev + 2);
+        if (!FILL) {
+            const bool ok = st == MJX_AW_OK;
+            V.counts[4 * g] = st;
+            V.counts[4 * g + 1] = ok ? n_ev + 2 : 0;
+            V.counts[4 * g + 2] = ok ? n_ky : 0;
+            V.counts[4 * g + 3] = ok ? n_ho : 0;
+        }
+    }
+}
+
 static bool mw_view(MwView& V, int n_games, const uint64_t* words, const int32_t* lens, int log_cap, const int32_t* bounds, int n_steps,
                     int key_steps, const int64_t* rec_key, const int32_t* rec_info, const uint64_t* rec_mask, const float* rec_q,
                     const int64_t* rec_i64, long long n_rec) {
@@ -1657,6 +1718,38 @@ int mjx_mjai_render_fill_dev(int n_games, const uint64_t* words, const int32_t* 
         return fail(MJX_ERR_ARG, "mjx_mjai_render_fill_dev: bad arguments");
     V.status = const_cast<int32_t*>(status); V.off = off; V.g0 = g0; V.g1 = g1; V.out = out; V.out_cap = out_cap;
     k_mjai_render<true><<<(g1 - g0 + MW_WARPS - 1) / MW_WARPS, MW_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+// ---- arena event words -> replay arrays (k_arena_words)
+int mjx_arena_words_count_dev(int n_games, const uint64_t* words, const int32_t* lens, long long pitch, int log_cap,
+                              int32_t* counts, void* stream) {
+    if (n_games <= 0 || !words || !lens || log_cap <= 0 || pitch < log_cap || !counts)
+        return fail(MJX_ERR_ARG, "mjx_arena_words_count_dev: bad arguments");
+    AwView V{};
+    V.words = words; V.lens = lens; V.pitch = pitch; V.log_cap = log_cap; V.n_games = n_games; V.counts = counts;
+    k_arena_words<false><<<(n_games + AW_WARPS - 1) / AW_WARPS, AW_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+int mjx_arena_words_fill_dev(int n_games, const uint64_t* words, const int32_t* lens, long long pitch, int log_cap, int augment,
+                             const int32_t* counts, const int32_t* ev_off, const int32_t* ky_off, const int32_t* hora_off,
+                             uint64_t* hdr, int32_t* lines, long long n_hdr, uint64_t* kyoku, long long n_kyoku_words,
+                             uint64_t* hora_payload, long long n_hora_words, int32_t* deltas, uint8_t* has_deltas, void* stream) {
+    if (n_games <= 0 || !words || !lens || log_cap <= 0 || pitch < log_cap || !counts || !ev_off || !ky_off || !hora_off ||
+        n_hdr < 0 || (n_hdr > 0 && (!hdr || !lines || !deltas || !has_deltas)) || n_kyoku_words < 0 ||
+        n_kyoku_words % REPLAY_KYOKU_WORDS || (n_kyoku_words > 0 && !kyoku) || n_hora_words < 0 || n_hora_words % MJX_HORA_WORDS ||
+        (n_hora_words > 0 && !hora_payload))
+        return fail(MJX_ERR_ARG, "mjx_arena_words_fill_dev: bad arguments");
+    AwView V{};
+    V.words = words; V.lens = lens; V.pitch = pitch; V.log_cap = log_cap; V.n_games = n_games; V.augment = augment;
+    V.counts = const_cast<int32_t*>(counts);
+    V.ev_off = ev_off; V.ky_off = ky_off; V.hora_off = hora_off;
+    V.hdr = hdr; V.lines = lines; V.n_hdr = n_hdr; V.kyoku = kyoku; V.n_kyoku = n_kyoku_words / REPLAY_KYOKU_WORDS;
+    V.hora = hora_payload; V.n_hora = n_hora_words / MJX_HORA_WORDS; V.deltas = deltas; V.has_deltas = has_deltas;
+    k_arena_words<true><<<(n_games + AW_WARPS - 1) / AW_WARPS, AW_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
     CU(cudaGetLastError());
     return MJX_OK;
 }

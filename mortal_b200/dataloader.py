@@ -184,9 +184,13 @@ class FileDatasetsIter:
         for start_idx in range(0, len(self.file_list), self.file_batch_size):
             yield self._populate(self.file_list[start_idx:start_idx + self.file_batch_size])
 
+    def _load(self, file_list):
+        """the Gameplays of a file batch (GameplayLoader.load_gz_log_files)"""
+        return self.loader.load_gz_log_files(file_list)
+
     def _populate(self, file_list):
         """load a file batch into the store (keeping the rows not batched yet) -> its sample count"""
-        data = self.loader.load_gz_log_files(file_list)
+        data = self._load(file_list)
         dev = self.device
         with torch.cuda.device(dev):
             jobs, new = gameplay_targets(data, self.reward_calc)

@@ -260,7 +260,31 @@ class GameplayLoader:
                 b, e = (int(x) for x in D.counts[slot[k], 4:6])
                 firsts.append(json.loads(logs[k].blob[b:e].decode("utf-8")))
         players = [self._players(f.get("names", ["", "", "", ""])) for f in firsts]
-        # the jobs: the decoded arrays on the device, the host-encoded logs' words and payloads appended after them
+        jobs = self._device_jobs(D, slot, games, players)
+
+        def grps():
+            out = []
+            for g in range(n):
+                if g in on_host:
+                    out.append(Grp.load_events(games[g]))
+                    continue
+                grp = G.grp(D, slot[g])
+                if grp is None:  # k_grp_logs declined: the host raises its exception for this log
+                    ev = dataset_codec.parse_log(logs[g].host_text())
+                    grp = Grp.load_events(dataset_codec.augment_events(ev) if self.augmented else ev)
+                out.append(grp)
+            return out
+
+        return self._replay(jobs, firsts, grps)
+
+    def _device_jobs(self, D, slot, games, players):
+        """the replay jobs of a batch of logs: log g is decoded log slot[g] of D (device arrays), or else games[g], its events
+        encoded on the host; players[g] = its selected seats. The decoded arrays stay on the device, the host-encoded logs' words
+        and payloads are appended after them."""
+        import torch
+
+        n = len(players)
+        on_host = set(games)
         dev = torch.device("cuda", self.device)
         hdr = [D.hdr] if D is not None else []
         kyoku = [D.kyoku] if D is not None else []
@@ -282,16 +306,42 @@ class GameplayLoader:
         jobs = dict(hdr=cat(hdr), kyoku=cat(kyoku), ev_off=np.array(ev_off, dtype=np.int32), ev_cnt=np.array(ev_cnt, dtype=np.int32),
                     ky_off=np.array(ky_off, dtype=np.int32), players=np.array(pids, dtype=np.uint8),
                     job_game=np.array(job_game, dtype=np.int32))
+        return jobs
+
+    def load_games(self, games, idx=None):
+        """load_gz_log_files over the written logs of self-play games idx (default all) of a selfplay.SelfPlayGames, without the
+        logs: the arena's words are converted on the device (selfplay.decode_games), scored by k_grp_logs and replayed. Needs the
+        loader's device path (oracle=False, or trust_seed=True)."""
+        import torch
+
+        from . import _lib
+        from .selfplay import decode_games
+
+        if self.oracle and not self.trust_seed:
+            raise ValueError("load_games: oracle=True needs trust_seed=True (the unseen tiles of a random fill come from the host path)")
+        idx = list(range(len(games))) if idx is None else [int(i) for i in idx]
+        if not idx:
+            return []
+        with torch.cuda.device(self.device):
+            _lib.init(self.device)
+            D = decode_games(games, idx, augment=self.augmented, device=self.device)
+            G = _grp_run(D, self.device)
+        for j in range(len(idx)):
+            if G.first_type[j] != dataset_codec.START_GAME or D.ev_cnt[j] < 4:
+                raise ValueError("empty or invalid game log")
+        firsts = [games.first_event(g) for g in idx]
+        players = [self._players(f["names"]) for f in firsts]
+        jobs = self._device_jobs(D, {j: j for j in range(len(idx))}, {}, players)
 
         def grps():
             out = []
-            for g in range(n):
-                if g in on_host:
-                    out.append(Grp.load_events(games[g]))
-                    continue
-                grp = G.grp(D, slot[g])
-                if grp is None:  # k_grp_logs declined: the host raises its exception for this log
-                    ev = dataset_codec.parse_log(logs[g].host_text())
+            for j, g in enumerate(idx):
+                grp = G.grp(D, j)
+                if grp is None:  # k_grp_logs declined: the host raises its exception for this game
+                    from .mjai_log import decode_events
+
+                    n = int(games.lens[g])
+                    ev = [firsts[j]] + decode_events(games.words[g, :n].cpu().numpy().view(np.uint64)) + [{"type": "end_game"}]
                     grp = Grp.load_events(dataset_codec.augment_events(ev) if self.augmented else ev)
                 out.append(grp)
             return out

@@ -127,9 +127,9 @@ class _Part:
         if arena.record_grp and hasattr(env, "enable_grp"):
             env.enable_grp()
         self.meta_rec = None
-        if arena.log_dir is not None:
+        if arena.log_dir is not None or arena.record_games:
             env.enable_log()
-            if arena.log_meta:
+            if arena.log_dir is not None and arena.log_meta:
                 # CUDA environments keep the records on the device (k_meta_record); others, and the host writer, use _MetaRecorder
                 from ..mjai_write import DeviceMetaRecorder
 
@@ -374,6 +374,8 @@ class _Arena:
         self.last_log_timing = None   # seconds per stage of the device log writer (count, fill_d2h, gzip_wait) of the last run
         self.record_grp = False  # keep the per-kyoku GRP features of every game (read on device, no logs): last_grp
         self.last_grp = None
+        self.record_games = False  # keep every game's event words on the device (no files needed): last_games, a SelfPlayGames
+        self.last_games = None
         self.pipeline = True    # play the batch as two half-batches stepped alternately (see the module docstring)
         self.pipeline_device_engines = False  # the same for device engines (env kernels of one half under the other half's forward)
         self.max_cycles = 0     # test hook: stop after this many BatchGame::run cycles (0 = play every table to the end)
@@ -388,6 +390,7 @@ class _Arena:
     def _run(self, challenger, champion, seed_start, seed_count):
         import torch
 
+        self.last_games = None  # set again below when record_games is on; never a previous run's games
         if challenger is champion:
             agents = [_adapt(challenger)] * 2
         else:
@@ -444,6 +447,8 @@ class _Arena:
 
                 feats = [f for p in parts for f in p.env.read_grp()]
                 self.last_grp = [Grp(feats[g], [int(x) for x in res["ranks"][g]], [int(x) for x in res["scores"][g]]) for g in range(n)]
+            if self.record_games:  # copied out of the environments before they are closed
+                self.last_games = self._games(parts, agents, per, res)
             sp_overflows = sum(p.env.sp_overflows() for p in parts)
             self.last_stats = dict(cycles=max(p.cycles for p in parts), table_steps=int(res["steps"].sum()), sp_overflows=sp_overflows,
                                    parts=len(parts), launches=sum(p.env.launch_count() for p in parts if hasattr(p.env, "launch_count")))
@@ -463,6 +468,30 @@ class _Arena:
             bad = int(np.nonzero(res["err"])[0][0])
             raise RuntimeError(f"table {bad} failed with mjx error code {int(res['err'][bad])}")
         return res
+
+    def _games(self, parts, agents, per, res):
+        """the parts' games as a selfplay.SelfPlayGames: words and lengths copied device to device, names and seeds as the log
+        writer writes them (CUDA environments; others are copied from the host)"""
+        import torch
+
+        from ..selfplay import SelfPlayGames
+
+        agent_names = [str(getattr(a, "name", "NoName")) for a in agents]
+        out = []
+        for p in parts:
+            names = [[agent_names[0] if p.ic_host[g % per, seat] else agent_names[1] for seat in range(4)] for g in range(p.n)]
+            seeds = [(int(p.nonces[g]), int(p.keys[g])) for g in range(p.n)]
+            lo = p.offset
+            if isinstance(p.env, BatchEnv):
+                with torch.cuda.device(p.dev):
+                    if p.stream is not None:
+                        torch.cuda.current_stream(p.dev).wait_stream(p.stream)
+                    words, lens = p.env.log_words.clone(), p.env.log_len.clone()
+            else:
+                w, ln = p.env.read_log()
+                words, lens = torch.from_numpy(w.view(np.int64)), torch.from_numpy(ln)
+            out.append(SelfPlayGames(words, lens, words.shape[1], names, seeds, res["ranks"][lo:lo + p.n], res["scores"][lo:lo + p.n]))
+        return SelfPlayGames.concat(out)
 
     def _write_logs(self, parts, agents, per):
         """The parts' logs, in part and game order. CUDA environments render the text on the device (mortal_b200.mjai_write) and

@@ -1,4 +1,5 @@
-"""mortal/train.py's offline trainer on the device: `python -m mortal_b200.train [CONFIG]`, or `train(config, steps=None)`.
+"""mortal/train.py's trainer on the device: `python -m mortal_b200.train [CONFIG]`, or `train(config, steps=None)` offline and
+`train_online(config, rounds=None, steps=None)` online (`main()` runs the one `control.online` selects).
 
 The loop of the reference's train(): batches from the device `FileDatasetsIter` (rewards from the `[grp]` GRP, as
 mortal/dataloader.py:41-43 loads it), the Brain's training forward as fused kernels around cuDNN convolutions
@@ -12,9 +13,20 @@ the reference's state file: `mortal` in mortal/model.py's key layout, `current_d
 ordered by the reference's sorted parameter names, so the optimizer state lines up index for index), `scheduler`, `scaler`,
 `steps`, `timestamp`, `best_perf`, `config`. State files move between the two trainers both ways.
 
+Online training replaces the reference's parameter server and self-play clients with one sequential loop in one process, the
+reference's `force_sequential = true`. Each round plays `player.TrainPlayer.train_play_games` sessions with the current parameters
+until at least `[online.server] capacity` games are held, logging each session's rankings and the `[online] history_window`
+moving average as mortal/client.py does. It then runs one `selfplay.SelfPlayDatasetsIter` over those games (the trainee's seats,
+the `[dataset]` flags), which yields what FileDatasetsIter yields over their written logs, so no log is written. The step uses the
+online loss, dqn + next_rank * next_rank_weight with no CQL term (mortal/train.py:236-238), and saves and test-plays as offline.
+Resuming from a state saved offline loads the weights, scaler, best_perf and steps, and starts a fresh optimizer and scheduler
+(mortal/train.py:106-118). These keys are read and have no effect: `submit_every` (no client plays during training),
+`force_sequential` (the loop is sequential), `[online.remote]`, `buffer_dir` and `drain_dir` (no files or sockets), and
+`[online] enable_compile`. The reference exits after a test play and respawns the trainer, a workaround for a hang in its
+process model; this loop simply continues.
+
 Differences from the reference, stated rather than hidden:
-- `online = true` raises ValueError: online training needs the reference's parameter server and self-play clients (submit_param,
-  drain, TrainPlayer), which are not built.
+- `train()` raises ValueError for `online = true`: the online loop is `train_online`.
 - Version 1 raises ValueError: its Brain returns (mu, logsig), which the reference's train.py cannot train either.
 - Oracle brains are not supported: train.py never passes invisible_obs.
 - `enable_compile` is read and not applied; `num_workers` has no effect (the sample stream is the in-process one, as in
@@ -28,6 +40,7 @@ from __future__ import annotations
 import gzip
 import json
 import logging
+import os
 import shutil
 import sys
 from datetime import datetime
@@ -36,6 +49,7 @@ from itertools import chain
 from os import path
 
 import torch
+import numpy as np
 from torch import nn, optim
 from torch.amp import GradScaler
 from torch.nn.utils import clip_grad_norm_
@@ -50,11 +64,28 @@ BEST_PERF = {"avg_rank": 4.0, "avg_pt": -135.0}
 
 
 def check_config(config):
-    """ValueError for what this trainer does not build (module docstring), before anything touches the device"""
+    """ValueError for what the offline trainer does not run (module docstring), before anything touches the device"""
+    if config["control"].get("online", False):
+        raise ValueError("online = true: online training runs in train_online(config), not train()")
+    _check_common(config)
+
+
+def check_online_config(config):
+    """ValueError for an online config train_online cannot run, before anything touches the device"""
+    _check_common(config)
+    profile = os.environ.get("TRAIN_PLAY_PROFILE", "default")
+    play = config.get("train_play", {}).get(profile)
+    if play is None:
+        raise ValueError(f"no [train_play.{profile}] profile for the trainee's self-play (TRAIN_PLAY_PROFILE selects it)")
+    if play["games"] < 4:
+        raise ValueError(f"[train_play.{profile}] games must be at least 4 (one seed plays 4 games), got {play['games']}")
+    capacity = config["online"]["server"]["capacity"]
+    if capacity < 1:
+        raise ValueError(f"[online.server] capacity must be at least 1, got {capacity}")
+
+
+def _check_common(config):
     control = config["control"]
-    if control.get("online", False):
-        raise ValueError("online training is not supported: it needs the reference's parameter server and self-play clients "
-                         "(submit_param, drain, TrainPlayer)")
     version = control["version"]
     if version == 1:
         raise ValueError("version 1 cannot be trained: its Brain returns (mu, logsig), which mortal/train.py cannot train either")
@@ -120,184 +151,269 @@ def _player_names(ds):
     return names
 
 
+class _Trainer:
+    """The models, optimizer, scheduler and scaler of mortal/train.py's train(), resumed from the state file, and its per-batch
+    step with the saves and test plays (online: the loss has no CQL term)."""
+
+    def __init__(self, config, online: bool):
+        control = config["control"]
+        self.config, self.online = config, online
+        self.version = version = control["version"]
+        self.batch_size, self.opt_step_every = control["batch_size"], control["opt_step_every"]
+        self.save_every, self.test_every = control["save_every"], control["test_every"]
+        self.test_games = config["test_play"]["games"]
+        self.min_q_weight = config["cql"]["min_q_weight"]
+        self.next_rank_weight = config["aux"]["next_rank_weight"]
+        self.gamma = config["env"]["gamma"]
+        self.max_grad_norm = config["optim"]["max_grad_norm"]
+        self.enable_amp = control["enable_amp"]
+        _ = control.get("enable_compile", False)  # read, not applied (module docstring)
+
+        device = torch.device(control["device"])
+        if device.type != "cuda":
+            raise ValueError(f"the trainer runs on a CUDA device, got {device}")
+        self.device = device = torch.device("cuda", device.index if device.index is not None else torch.cuda.current_device())
+        self.cudnn_benchmark = control.get("enable_cudnn_benchmark", False)
+        torch.backends.cudnn.benchmark = self.cudnn_benchmark
+
+        self.mortal = mortal = Brain(version=version, **config["resnet"]).to(device)
+        self.dqn = dqn = DQN(version=version).to(device)
+        self.aux_net = aux_net = AuxNet((4,)).to(device)
+        logging.info(f"version: {version}")
+        for name, m in (("mortal", mortal), ("dqn", dqn), ("aux", aux_net)):
+            logging.info(f"{name} params: {sum(p.numel() for p in m.parameters() if p.requires_grad):,}")
+        mortal.freeze_bn(config["freeze_bn"]["mortal"])
+
+        self.optimizer = make_optimizer(mortal, dqn, aux_net, config["optim"])
+        self.scheduler = LinearWarmUpCosineAnnealingLR(self.optimizer, **config["optim"]["scheduler"])
+        self.scaler = GradScaler(device.type, enabled=self.enable_amp)
+        from .player import TestPlayer
+
+        self.test_player = TestPlayer(config)
+        self.best_perf = dict(BEST_PERF)
+
+        self.total = 0
+        self.state_file, self.best_state_file = control["state_file"], control["best_state_file"]
+        if path.exists(self.state_file):
+            state = torch.load(self.state_file, weights_only=True, map_location=device)
+            logging.info(f"loaded: {datetime.fromtimestamp(state['timestamp']).strftime('%Y-%m-%d %H:%M:%S')}")
+            load_mortal_state(mortal, state["mortal"])
+            dqn.load_state_dict(state["current_dqn"])
+            aux_net.load_state_dict(state["aux_net"])
+            if not online or state["config"]["control"].get("online", False):  # mortal/train.py:113-115
+                self.optimizer.load_state_dict(state["optimizer"])
+                self.scheduler.load_state_dict(state["scheduler"])
+            self.scaler.load_state_dict(state["scaler"])
+            self.best_perf = state["best_perf"]
+            self.total = state["steps"]
+        self.optimizer.zero_grad(set_to_none=True)
+        logging.info(f"device: {device} ({torch.cuda.get_device_name(device)})")
+
+        zero = lambda: torch.zeros((), dtype=torch.float64, device=device)
+        self._zero = zero
+        self.stats = {k: zero() for k in ("dqn_loss", "cql_loss", "next_rank_loss")}
+        self.all_q = torch.zeros((self.save_every, self.batch_size), dtype=torch.float32, device=device)
+        self.all_q_target = torch.zeros_like(self.all_q)
+        self.bad_steps = torch.zeros(self.save_every, dtype=torch.int32, device=device)
+        self.idx = 0
+
+    def check_actions(self):
+        """ValueError naming the first step since the last check whose batch had an action outside its mask"""
+        hit = torch.nonzero(self.bad_steps[:self.idx]).flatten().tolist()
+        if hit:
+            raise ValueError(f"step {self.total - self.idx + hit[0] + 1}: an action of the batch is not legal in its mask")
+
+    def step(self, obs, actions, masks, steps_to_done, kyoku_rewards, player_ranks):
+        """one training step on a full batch, then the save and the test play when they are due"""
+        mortal, dqn, aux_net = self.mortal, self.dqn, self.aux_net
+        with torch.autocast(self.device.type, enabled=self.enable_amp):
+            phi = mortal.forward_train(obs)
+            v, a = dqn.heads(phi)
+            next_rank_logits, = aux_net(phi)
+            dqn_loss, cql_loss, next_rank_loss, q, q_target, bad = train_ops.dqn_losses(
+                v, a, next_rank_logits, masks, actions, steps_to_done, kyoku_rewards, player_ranks, self.gamma)
+            if self.online:  # mortal/train.py:236-238: no CQL term (its output gets no gradient)
+                loss = dqn_loss + next_rank_loss * self.next_rank_weight
+            else:
+                loss = dqn_loss + cql_loss * self.min_q_weight + next_rank_loss * self.next_rank_weight
+        self.scaler.scale(loss / self.opt_step_every).backward()
+
+        idx = self.idx
+        with torch.no_grad():
+            self.stats["dqn_loss"] += dqn_loss
+            if not self.online:
+                self.stats["cql_loss"] += cql_loss
+            self.stats["next_rank_loss"] += next_rank_loss
+            self.all_q[idx] = q
+            self.all_q_target[idx] = q_target
+            self.bad_steps[idx] = bad
+        self.total += 1
+        self.idx += 1
+        if self.idx % self.opt_step_every == 0:
+            if self.max_grad_norm > 0:
+                self.scaler.unscale_(self.optimizer)
+                clip_grad_norm_(chain.from_iterable(g["params"] for g in self.optimizer.param_groups), self.max_grad_norm)
+            self.scaler.step(self.optimizer)
+            self.scaler.update()
+            self.optimizer.zero_grad(set_to_none=True)
+        self.scheduler.step()
+        if self.total % self.save_every == 0:
+            self._save()
+
+    def _save(self):
+        total, test_every, stats = self.total, self.test_every, self.stats
+        self.check_actions()
+        n = self.save_every
+        cql = "" if self.online else f" cql_loss {(stats['cql_loss'] / n).item():.6f}"
+        logging.info(f"steps {total:,}: dqn_loss {(stats['dqn_loss'] / n).item():.6f}{cql} "
+                     f"next_rank_loss {(stats['next_rank_loss'] / n).item():.6f} lr {self.scheduler.get_last_lr()[0]:.4e} "
+                     f"q {self.all_q.mean().item():.6f} q_target {self.all_q_target.mean().item():.6f}")
+        for k in stats:
+            stats[k] = self._zero()
+        self.idx = 0
+        logging.info(f"total steps: {total:,} (~{(test_every - total % test_every) % test_every:,})")
+        state = {
+            "mortal": mortal_state_dict(self.mortal),
+            "current_dqn": self.dqn.state_dict(),
+            "aux_net": self.aux_net.state_dict(),
+            "optimizer": self.optimizer.state_dict(),
+            "scheduler": self.scheduler.state_dict(),
+            "scaler": self.scaler.state_dict(),
+            "steps": total,
+            "timestamp": datetime.now().timestamp(),
+            "best_perf": self.best_perf,
+            "config": self.config,
+        }
+        torch.save(state, self.state_file)
+
+        if total % test_every == 0:
+            best_perf = self.best_perf
+            stat = self.test_player.test_play(self.test_games // 4, self.mortal, self.dqn, self.device)
+            self.mortal.train()
+            self.dqn.train()
+            avg_pt = stat.avg_pt([90, 45, 0, -135])  # for display only, never used in training
+            better = avg_pt >= best_perf["avg_pt"] and stat.avg_rank <= best_perf["avg_rank"]
+            if better:
+                past_best = best_perf.copy()
+                best_perf["avg_pt"] = avg_pt
+                best_perf["avg_rank"] = stat.avg_rank
+            logging.info(f"avg rank: {stat.avg_rank:.6}")
+            logging.info(f"avg pt: {avg_pt:.6}")
+            logging.info("test play: rank 1/2/3/4 {:.4f} {:.4f} {:.4f} {:.4f}; agari {:.4f} houjuu {:.4f} fuuro {:.4f} "
+                         "riichi {:.4f}; point per agari {:.1f} (riichi {:.1f}, fuuro {:.1f}, dama {:.1f}), per houjuu {:.1f}, "
+                         "per round {:.1f}; jun agari {:.2f} houjuu {:.2f} riichi {:.2f}; after riichi agari {:.4f} houjuu "
+                         "{:.4f}, chasing {:.4f}, chased {:.4f}, riichi point {:.1f}; after fuuro agari {:.4f} houjuu {:.4f}, "
+                         "fuuro num {:.4f}, fuuro point {:.1f}".format(
+                             stat.rank_1_rate, stat.rank_2_rate, stat.rank_3_rate, stat.rank_4_rate, stat.agari_rate,
+                             stat.houjuu_rate, stat.fuuro_rate, stat.riichi_rate, stat.avg_point_per_agari,
+                             stat.avg_point_per_riichi_agari, stat.avg_point_per_fuuro_agari, stat.avg_point_per_dama_agari,
+                             stat.avg_point_per_houjuu, stat.avg_point_per_round, stat.avg_agari_jun, stat.avg_houjuu_jun,
+                             stat.avg_riichi_jun, stat.agari_rate_after_riichi, stat.houjuu_rate_after_riichi,
+                             stat.chasing_riichi_rate, stat.riichi_chased_rate, stat.avg_riichi_point,
+                             stat.agari_rate_after_fuuro, stat.houjuu_rate_after_fuuro, stat.avg_fuuro_num, stat.avg_fuuro_point))
+            if better:
+                torch.save(state, self.state_file)
+                logging.info(f"a new record has been made, pt: {past_best['avg_pt']:.4} -> {best_perf['avg_pt']:.4}, "
+                             f"rank: {past_best['avg_rank']:.4} -> {best_perf['avg_rank']:.4}, saving to {self.best_state_file}")
+                shutil.copy(self.state_file, self.best_state_file)
+
+
+def _load_grp(config):
+    grp = GRP(**config["grp"]["network"])
+    grp.load_state_dict(torch.load(config["grp"]["state_file"], weights_only=True, map_location=torch.device("cpu"))["model"])
+    return grp
+
+
 def train(config, steps=None):
     """mortal/train.py train() over the whole config (dict), offline: one pass over the file list, as the reference runs. `steps`
     bounds this call to that many training steps (None: until the data ends). Returns (brain, dqn, aux_net, optimizer, total
     steps)."""
     check_config(config)
-    control = config["control"]
-    version = control["version"]
-    batch_size, opt_step_every = control["batch_size"], control["opt_step_every"]
-    save_every, test_every = control["save_every"], control["test_every"]
-    test_games = config["test_play"]["games"]
-    min_q_weight = config["cql"]["min_q_weight"]
-    next_rank_weight = config["aux"]["next_rank_weight"]
-    gamma, pts = config["env"]["gamma"], config["env"]["pts"]
+    T = _Trainer(config, online=False)
     ds = config["dataset"]
-    optim_cfg = config["optim"]
-    max_grad_norm = optim_cfg["max_grad_norm"]
-    enable_amp = control["enable_amp"]
-    _ = control.get("enable_compile", False)  # read, not applied (module docstring)
-
-    device = torch.device(control["device"])
-    if device.type != "cuda":
-        raise ValueError(f"the trainer runs on a CUDA device, got {device}")
-    device = torch.device("cuda", device.index if device.index is not None else torch.cuda.current_device())
-    torch.backends.cudnn.benchmark = control.get("enable_cudnn_benchmark", False)
-
-    mortal = Brain(version=version, **config["resnet"]).to(device)
-    dqn = DQN(version=version).to(device)
-    aux_net = AuxNet((4,)).to(device)
-    logging.info(f"version: {version}")
-    for name, m in (("mortal", mortal), ("dqn", dqn), ("aux", aux_net)):
-        logging.info(f"{name} params: {sum(p.numel() for p in m.parameters() if p.requires_grad):,}")
-    mortal.freeze_bn(config["freeze_bn"]["mortal"])
-
-    optimizer = make_optimizer(mortal, dqn, aux_net, optim_cfg)
-    scheduler = LinearWarmUpCosineAnnealingLR(optimizer, **optim_cfg["scheduler"])
-    scaler = GradScaler(device.type, enabled=enable_amp)
-    from .player import TestPlayer
-
-    test_player = TestPlayer(config)
-    best_perf = dict(BEST_PERF)
-
-    total = 0
-    state_file, best_state_file = control["state_file"], control["best_state_file"]
-    if path.exists(state_file):
-        state = torch.load(state_file, weights_only=True, map_location=device)
-        logging.info(f"loaded: {datetime.fromtimestamp(state['timestamp']).strftime('%Y-%m-%d %H:%M:%S')}")
-        load_mortal_state(mortal, state["mortal"])
-        dqn.load_state_dict(state["current_dqn"])
-        aux_net.load_state_dict(state["aux_net"])
-        optimizer.load_state_dict(state["optimizer"])
-        scheduler.load_state_dict(state["scheduler"])
-        scaler.load_state_dict(state["scaler"])
-        best_perf = state["best_perf"]
-        total = state["steps"]
-    optimizer.zero_grad(set_to_none=True)
-    logging.info(f"device: {device} ({torch.cuda.get_device_name(device)})")
-
-    grp = GRP(**config["grp"]["network"])
-    grp.load_state_dict(torch.load(config["grp"]["state_file"], weights_only=True, map_location=torch.device("cpu"))["model"])
+    grp = _load_grp(config)
     player_names_set = _player_names(ds)
     logging.info(f"loaded {len(player_names_set):,} players")
     file_list = _file_list(ds, player_names_set)
     logging.info(f"file list size: {len(file_list):,}")
-    logging.info(f"total steps: {total:,} (~{(test_every - total % test_every) % test_every:,})")
-    file_data = FileDatasetsIter(version, file_list, pts, file_batch_size=ds["file_batch_size"], reserve_ratio=ds["reserve_ratio"],
-                                 player_names=list(player_names_set), num_epochs=ds["num_epochs"],
+    logging.info(f"total steps: {T.total:,} (~{(T.test_every - T.total % T.test_every) % T.test_every:,})")
+    file_data = FileDatasetsIter(T.version, file_list, config["env"]["pts"], file_batch_size=ds["file_batch_size"],
+                                 reserve_ratio=ds["reserve_ratio"], player_names=list(player_names_set), num_epochs=ds["num_epochs"],
                                  enable_augmentation=ds["enable_augmentation"], augmented_first=ds["augmented_first"], grp=grp,
-                                 batch_size=batch_size, device=device.index)
-
-    zero = lambda: torch.zeros((), dtype=torch.float64, device=device)
-    stats = {k: zero() for k in ("dqn_loss", "cql_loss", "next_rank_loss")}
-    all_q = torch.zeros((save_every, batch_size), dtype=torch.float32, device=device)
-    all_q_target = torch.zeros_like(all_q)
-    bad_steps = torch.zeros(save_every, dtype=torch.int32, device=device)
-    idx = 0
-
-    def check_actions(first_step):
-        """ValueError naming the first step since the last check whose batch had an action outside its mask"""
-        hit = torch.nonzero(bad_steps[:idx]).flatten().tolist()
-        if hit:
-            raise ValueError(f"step {first_step + hit[0] + 1}: an action of the batch is not legal in its mask")
-
+                                 batch_size=T.batch_size, device=T.device.index)
     done = 0
-    for obs, actions, masks, steps_to_done, kyoku_rewards, player_ranks in file_data:
+    for batch in file_data:
         if steps is not None and done >= steps:
             break
-        if obs.shape[0] != batch_size:
+        if batch[0].shape[0] != T.batch_size:
             continue  # a final short batch is not trained on (mortal/train.py:389-422)
-        with torch.autocast(device.type, enabled=enable_amp):
-            phi = mortal.forward_train(obs)
-            v, a = dqn.heads(phi)
-            next_rank_logits, = aux_net(phi)
-            dqn_loss, cql_loss, next_rank_loss, q, q_target, bad = train_ops.dqn_losses(
-                v, a, next_rank_logits, masks, actions, steps_to_done, kyoku_rewards, player_ranks, gamma)
-            loss = dqn_loss + cql_loss * min_q_weight + next_rank_loss * next_rank_weight
-        scaler.scale(loss / opt_step_every).backward()
-
-        with torch.no_grad():
-            stats["dqn_loss"] += dqn_loss
-            stats["cql_loss"] += cql_loss
-            stats["next_rank_loss"] += next_rank_loss
-            all_q[idx] = q
-            all_q_target[idx] = q_target
-            bad_steps[idx] = bad
-        total += 1
+        T.step(*batch)
         done += 1
-        idx += 1
-        if idx % opt_step_every == 0:
-            if max_grad_norm > 0:
-                scaler.unscale_(optimizer)
-                clip_grad_norm_(chain.from_iterable(g["params"] for g in optimizer.param_groups), max_grad_norm)
-            scaler.step(optimizer)
-            scaler.update()
-            optimizer.zero_grad(set_to_none=True)
-        scheduler.step()
+    T.check_actions()
+    return T.mortal, T.dqn, T.aux_net, T.optimizer, T.total
 
-        if total % save_every == 0:
-            check_actions(total - idx)
-            n = save_every
-            logging.info(f"steps {total:,}: dqn_loss {(stats['dqn_loss'] / n).item():.6f} cql_loss {(stats['cql_loss'] / n).item():.6f} "
-                         f"next_rank_loss {(stats['next_rank_loss'] / n).item():.6f} lr {scheduler.get_last_lr()[0]:.4e} "
-                         f"q {all_q.mean().item():.6f} q_target {all_q_target.mean().item():.6f}")
-            for k in stats:
-                stats[k] = zero()
-            idx = 0
-            logging.info(f"total steps: {total:,} (~{(test_every - total % test_every) % test_every:,})")
-            state = {
-                "mortal": mortal_state_dict(mortal),
-                "current_dqn": dqn.state_dict(),
-                "aux_net": aux_net.state_dict(),
-                "optimizer": optimizer.state_dict(),
-                "scheduler": scheduler.state_dict(),
-                "scaler": scaler.state_dict(),
-                "steps": total,
-                "timestamp": datetime.now().timestamp(),
-                "best_perf": best_perf,
-                "config": config,
-            }
-            torch.save(state, state_file)
 
-            if total % test_every == 0:
-                stat = test_player.test_play(test_games // 4, mortal, dqn, device)
-                mortal.train()
-                dqn.train()
-                avg_pt = stat.avg_pt([90, 45, 0, -135])  # for display only, never used in training
-                better = avg_pt >= best_perf["avg_pt"] and stat.avg_rank <= best_perf["avg_rank"]
-                if better:
-                    past_best = best_perf.copy()
-                    best_perf["avg_pt"] = avg_pt
-                    best_perf["avg_rank"] = stat.avg_rank
-                logging.info(f"avg rank: {stat.avg_rank:.6}")
-                logging.info(f"avg pt: {avg_pt:.6}")
-                logging.info("test play: rank 1/2/3/4 {:.4f} {:.4f} {:.4f} {:.4f}; agari {:.4f} houjuu {:.4f} fuuro {:.4f} "
-                             "riichi {:.4f}; point per agari {:.1f} (riichi {:.1f}, fuuro {:.1f}, dama {:.1f}), per houjuu {:.1f}, "
-                             "per round {:.1f}; jun agari {:.2f} houjuu {:.2f} riichi {:.2f}; after riichi agari {:.4f} houjuu "
-                             "{:.4f}, chasing {:.4f}, chased {:.4f}, riichi point {:.1f}; after fuuro agari {:.4f} houjuu {:.4f}, "
-                             "fuuro num {:.4f}, fuuro point {:.1f}".format(
-                                 stat.rank_1_rate, stat.rank_2_rate, stat.rank_3_rate, stat.rank_4_rate, stat.agari_rate,
-                                 stat.houjuu_rate, stat.fuuro_rate, stat.riichi_rate, stat.avg_point_per_agari,
-                                 stat.avg_point_per_riichi_agari, stat.avg_point_per_fuuro_agari, stat.avg_point_per_dama_agari,
-                                 stat.avg_point_per_houjuu, stat.avg_point_per_round, stat.avg_agari_jun, stat.avg_houjuu_jun,
-                                 stat.avg_riichi_jun, stat.agari_rate_after_riichi, stat.houjuu_rate_after_riichi,
-                                 stat.chasing_riichi_rate, stat.riichi_chased_rate, stat.avg_riichi_point,
-                                 stat.agari_rate_after_fuuro, stat.houjuu_rate_after_fuuro, stat.avg_fuuro_num, stat.avg_fuuro_point))
-                if better:
-                    torch.save(state, state_file)
-                    logging.info(f"a new record has been made, pt: {past_best['avg_pt']:.4} -> {best_perf['avg_pt']:.4}, "
-                                 f"rank: {past_best['avg_rank']:.4} -> {best_perf['avg_rank']:.4}, saving to {best_state_file}")
-                    shutil.copy(state_file, best_state_file)
-    check_actions(total - idx)
-    return mortal, dqn, aux_net, optimizer, total
+def train_online(config, rounds=None, steps=None):
+    """mortal/train.py with `online = true`, as one sequential loop in this process (module docstring). `rounds` bounds the call
+    to that many rounds of self-play + training, `steps` to that many training steps (None: no bound; the loop then runs until
+    interrupted). Returns (brain, dqn, aux_net, optimizer, total steps)."""
+    from .player import TrainPlayer
+    from .selfplay import SelfPlayDatasetsIter, SelfPlayGames
+
+    check_online_config(config)
+    online_cfg = config["online"]
+    server = online_cfg["server"]
+    capacity, history_window = server["capacity"], online_cfg["history_window"]
+    _ = (config["control"].get("submit_every"), server.get("force_sequential"), server.get("buffer_dir"),  # read, no effect
+         server.get("drain_dir"), online_cfg.get("remote"), online_cfg.get("enable_compile"))       # (module docstring)
+    T = _Trainer(config, online=True)
+    ds = config["dataset"]
+    grp = _load_grp(config)
+    train_player = TrainPlayer(config)
+    pts = np.array([90, 45, 0, -135])  # mortal/client.py:31, for the log lines only
+    history = []
+    done = rounds_done = 0
+    while (rounds is None or rounds_done < rounds) and (steps is None or done < steps):
+        held, n_games = [], 0
+        while n_games < capacity:  # mortal/client.py:54-65, one session at a time
+            rankings, games = train_player.train_play_games(T.mortal, T.dqn, T.device)
+            held.append(games)
+            n_games += len(games)
+            history.append(np.array(rankings))
+            if len(history) > history_window:
+                del history[0]
+            total_r = np.sum(history, axis=0)
+            logging.info(f"trainee rankings: {rankings} ({rankings @ np.arange(1, 5) / rankings.sum():.6}, "
+                         f"{rankings @ pts / rankings.sum():.6}pt)")
+            logging.info(f"last {len(history)} sessions: {total_r} ({total_r @ np.arange(1, 5) / total_r.sum():.6}, "
+                         f"{total_r @ pts / total_r.sum():.6}pt)")
+        games = SelfPlayGames.concat(held)
+        del held
+        logging.info(f"round {rounds_done + 1}: {len(games):,} games; total steps: {T.total:,} "
+                     f"(~{(T.test_every - T.total % T.test_every) % T.test_every:,})")
+        data = SelfPlayDatasetsIter(T.version, games, config["env"]["pts"], file_batch_size=ds["file_batch_size"],
+                                    reserve_ratio=ds["reserve_ratio"], player_names=["trainee"], num_epochs=ds["num_epochs"],
+                                    enable_augmentation=ds["enable_augmentation"], augmented_first=ds["augmented_first"], grp=grp,
+                                    batch_size=T.batch_size, device=T.device.index)
+        for batch in data:
+            if steps is not None and done >= steps:
+                break
+            if batch[0].shape[0] != T.batch_size:
+                continue  # a final short batch is not trained on (mortal/train.py:389-422)
+            T.step(*batch)
+            done += 1
+        del data, games  # the round's games are freed before the next round plays
+        rounds_done += 1
+    T.check_actions()
+    return T.mortal, T.dqn, T.aux_net, T.optimizer, T.total
 
 
 def main(argv=None):
     argv = sys.argv[1:] if argv is None else argv
     logging.basicConfig(level=logging.INFO, format="%(asctime)s %(levelname)s %(message)s")
     try:
-        train(load_config(argv[0] if argv else None))
+        config = load_config(argv[0] if argv else None)
+        (train_online if config["control"].get("online", False) else train)(config)
     except KeyboardInterrupt:
         pass
 
