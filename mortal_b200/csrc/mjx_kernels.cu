@@ -13,6 +13,7 @@
 #include "mjx_replay.cuh"
 #include "mjx_validate.cuh"
 #include "mjx_mjai.cuh"
+#include "mjx_inflate.cuh"
 #include "mjx_mjai_write.cuh"
 #include "mjx_selfplay.cuh"
 #include "mjx_stat.cuh"
@@ -1718,6 +1719,38 @@ int mjx_mjai_render_fill_dev(int n_games, const uint64_t* words, const int32_t* 
         return fail(MJX_ERR_ARG, "mjx_mjai_render_fill_dev: bad arguments");
     V.status = const_cast<int32_t*>(status); V.off = off; V.g0 = g0; V.g1 = g1; V.out = out; V.out_cap = out_cap;
     k_mjai_render<true><<<(g1 - g0 + MW_WARPS - 1) / MW_WARPS, MW_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+// ---- gzip members -> log text, key counts over the text (include/mjx_logio.h)
+int mjx_gunzip_dev(int n, const uint8_t* gz, long long n_gz, const int64_t* gz_off, uint8_t* out, long long n_out,
+                   const int64_t* out_off, int32_t* status, void* stream) {
+    if (n <= 0 || n_gz < 0 || (n_gz > 0 && !gz) || ((uintptr_t)gz & 7) || !gz_off || n_out < 0 || (n_out > 0 && !out) ||
+        !out_off || !status)
+        return fail(MJX_ERR_ARG, "mjx_gunzip_dev: bad arguments");
+    k_gunzip<<<(n + GZ_WARPS - 1) / GZ_WARPS, GZ_WARPS * 32, 0, (cudaStream_t)stream>>>(n, gz, n_gz, gz_off, out, n_out, out_off,
+                                                                                       status);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+int mjx_count_keys_dev(int n_logs, const uint8_t* text, long long n_bytes, const int64_t* log_off, const uint8_t* keys_host,
+                       const int32_t* key_off_host, int n_keys, int64_t* counts, void* stream) {
+    if (n_logs <= 0 || n_bytes < 0 || (n_bytes > 0 && !text) || !log_off || !keys_host || !key_off_host || n_keys < 1 ||
+        n_keys > MJX_COUNT_KEYS_MAX || !counts)
+        return fail(MJX_ERR_ARG, "mjx_count_keys_dev: bad arguments");
+    GzKeys K{};
+    K.n = n_keys;
+    for (int k = 0; k < n_keys; k++) {
+        const int len = key_off_host[k + 1] - key_off_host[k];
+        if (key_off_host[k] < 0 || len < 1 || len > MJX_COUNT_KEY_BYTES)
+            return fail(MJX_ERR_ARG, "mjx_count_keys_dev: key " + std::to_string(k) + " is empty or too long");
+        K.len[k] = len;
+        std::memcpy(K.b[k], keys_host + key_off_host[k], len);
+    }
+    k_count_keys<<<(n_logs + GZ_WARPS - 1) / GZ_WARPS, GZ_WARPS * 32, 0, (cudaStream_t)stream>>>(n_logs, text, n_bytes, log_off, K,
+                                                                                                counts);
     CU(cudaGetLastError());
     return MJX_OK;
 }

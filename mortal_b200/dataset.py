@@ -19,9 +19,10 @@ against the logged deal) and otherwise from the log plus a random fill of the un
 csrc/mjx_grp.cuh).
 
 With libmjx built, a CUDA device and a UTF-8 locale, `load_gz_log_files`, `load_logs` and `Grp.load_gz_log_files` decode the log
-text on the device (k_mjai_decode with the deltas output, csrc/mjx_mjai.cuh): the event words go to the replay without leaving
-the device, and the Grp of every log comes from k_grp_logs. A log the decoder declines, or one that is not UTF-8, is parsed by the
-host code below, and so is every log of a batch loaded with `oracle=True, trust_seed=False` (its hidden tiles are drawn from the
+text on the device (k_mjai_decode with the deltas output, csrc/mjx_mjai.cuh), the files' bytes gunzipped there first (k_gunzip,
+csrc/mjx_inflate.cuh): the event words go to the replay without leaving the device, and the Grp of every log comes from
+k_grp_logs. A file k_gunzip declines, a log the decoder declines, or one that is not UTF-8, is read and parsed by the host code
+below, and so is every log of a batch loaded with `oracle=True, trust_seed=False` (its hidden tiles are drawn from the
 caller's numpy `rng`). The results and the exceptions are those of the host code either way.
 """
 from __future__ import annotations
@@ -179,33 +180,44 @@ class GameplayLoader:
         return not (self.oracle and not self.trust_seed) and _logio.device_ready()
 
     def load_gz_log_files(self, gzip_filenames):
+        import torch
+
+        from . import _lib
+
         if not self._on_device():
             texts = []
             for fn in gzip_filenames:
                 texts.append(_read_gz_text(fn))
             return self._load_host(texts)
         paths = list(gzip_filenames)
-        with ThreadPoolExecutor(max(1, min(32, os.cpu_count() or 1, len(paths)))) as pool:  # zlib and file reads release the GIL
-            blobs = list(pool.map(_logio.read_gz, paths))
-        logs = []
-        for fn, b in zip(paths, blobs):
-            if b is None or not _logio.utf8_ok(b):  # the host reader raises its own exception (or reads the file after all)
-                logs.append(_Log(text=_read_gz_text(fn)))
-            else:
-                logs.append(_Log(blob=b))
-        return self._load_device(logs)
+        with ThreadPoolExecutor(max(1, min(32, os.cpu_count() or 1, len(paths)))) as pool, torch.cuda.device(self.device):
+            items = list(pool.map(_logio.read_gz_file, paths))  # file reads and zlib release the GIL
+            _lib.init(self.device)
+            T = _logio.stage(items, self.device, pool)  # a file it cannot take is read by the host reader
+        logs = [_Log(path=fn) for fn in paths]
+        for j, k in enumerate(T.files):
+            logs[k].slot = j
+        return self._load_device(logs, T)
 
     def load_logs(self, texts):
         """list of log texts -> list (per log) of list (per selected player) of Gameplay; all logs replayed as one batch"""
+        import torch
+
+        from . import _lib
+
         if not self._on_device():
             return self._load_host(texts)
-        logs = []
+        logs, blobs = [], []
         for t in texts:
+            logs.append(_Log(text=t))
             try:
-                logs.append(_Log(text=t, blob=t.encode("utf-8")))
+                blobs.append(t.encode("utf-8")); logs[-1].slot = len(blobs) - 1
             except UnicodeEncodeError:  # lone surrogates: not UTF-8, so the host decides
-                logs.append(_Log(text=t))
-        return self._load_device(logs)
+                pass
+        with torch.cuda.device(self.device):
+            _lib.init(self.device)
+            T = _logio.stage([(b, False) for b in blobs], self.device)
+        return self._load_device(logs, T)
 
     def _load_host(self, texts):
         """load_logs with every log parsed, encoded and scored on the host"""
@@ -222,27 +234,29 @@ class GameplayLoader:
         jobs = dataset_codec.build_jobs(games, players, walls)
         return self._replay(jobs, [ev[0] for ev in games], lambda: [Grp.load_events(ev) for ev in games])
 
-    def _load_device(self, logs):
-        """load_logs over _Log items: decoded on the device (module docstring), the rest through the host code; the checks and
-        exceptions come in the host path's order"""
+    def _load_device(self, logs, T):
+        """load_logs over _Log items whose texts are slots of T (a _logio.DeviceText): decoded on the device (module docstring),
+        the rest through the host code; the checks and exceptions come in the host path's order"""
         import torch
 
         from . import _lib
-        from .validate_logs import decode_dev
+        from .validate_logs import decode_dev_text
 
         n = len(logs)
-        dev_idx = [k for k, lg in enumerate(logs) if lg.blob is not None]
-        slot = {k: j for j, k in enumerate(dev_idx)}
-        D = G = None
+        slot = {k: lg.slot for k, lg in enumerate(logs) if lg.slot is not None}
+        D = G = keys = None
         with torch.cuda.device(self.device):
             _lib.init(self.device)
-            if dev_idx:
-                D = decode_dev([logs[k].blob for k in dev_idx], self.device, augment=self.augmented, deltas=True)
+            if slot:
+                D = decode_dev_text(T.text, T.log_off, self.device, augment=self.augmented, deltas=True, status=T.status)
                 G = _grp_run(D, self.device, with_types=self.augmented)
+                if self.augmented:
+                    keys = _logio.count_keys(T.text, T.log_off, [k for k, _ in _AUGMENTED_FIELDS], self.device)
         host = [k for k in range(n) if k not in slot or not D.accept[slot[k]] or
-                (self.augmented and not _augment_safe(logs[k].blob, G.types[slot[k]]))]
+                (self.augmented and not _augment_counts_safe(keys[slot[k]], G.types[slot[k]]))]
         on_host = set(host)
-        games = {k: dataset_codec.parse_log(logs[k].host_text()) for k in host}  # parse errors first, in log order
+        texts = {k: logs[k].host_text() for k in host}  # read errors first, then parse errors, in log order
+        games = {k: dataset_codec.parse_log(texts[k]) for k in host}
         if self.augmented:
             games = {k: dataset_codec.augment_events(games[k]) for k in host}
         for k in range(n):
@@ -252,13 +266,11 @@ class GameplayLoader:
                     raise ValueError("empty or invalid game log")
             elif G.first_type[slot[k]] != dataset_codec.START_GAME or D.ev_cnt[slot[k]] < 4:
                 raise ValueError("empty or invalid game log")
-        firsts = []
-        for k in range(n):  # the first event: names and seed (the decoder reports its line as a byte span)
-            if k in on_host:
-                firsts.append(games[k][0])
-            else:
-                b, e = (int(x) for x in D.counts[slot[k], 4:6])
-                firsts.append(json.loads(logs[k].blob[b:e].decode("utf-8")))
+        dev_logs = [k for k in range(n) if k not in on_host]  # the first event: names and seed (the decoder reports its line's bytes)
+        at = [slot[k] for k in dev_logs]
+        lines = _logio.spans(T.text, T.log_off, at, D.counts[at, 4], D.counts[at, 5], self.device) if at else []
+        first_line = dict(zip(dev_logs, lines))
+        firsts = [games[k][0] if k in on_host else json.loads(first_line[k].decode("utf-8")) for k in range(n)]
         players = [self._players(f.get("names", ["", "", "", ""])) for f in firsts]
         jobs = self._device_jobs(D, slot, games, players)
 
@@ -429,15 +441,15 @@ def _read_gz_text(fn):
 
 
 class _Log:
-    """one log of a device load: `blob` = its UTF-8 bytes for the decoder (None: the host parses it), `text` = the str the host
-    code parses (made from the blob as the host reader would, when needed)"""
+    """one log of a device load: `slot` = its text's slot in the load's _logio.DeviceText (None: the host parses it), `text` =
+    the str the host code parses, or `path` = the file the host reader reads it from when needed"""
 
-    def __init__(self, text=None, blob=None):
-        self.text, self.blob = text, blob
+    def __init__(self, text=None, path=None):
+        self.text, self.path, self.slot = text, path, None
 
     def host_text(self):
         if self.text is None:
-            self.text = _logio.host_text(self.blob)
+            self.text = _read_gz_text(self.path)
         return self.text
 
 
@@ -458,7 +470,12 @@ def _augment_safe(blob: bytes, types) -> bool:
     """whether every field augment_events rewrites sits on an event whose type the decoder checked it for: a key is never escaped
     in an accepted log, so it appears in the text at least once per event that has it (more often only inside other strings
     or values, which merely sends the log to the host); `types` = the log's event count per type"""
-    return all(blob.count(key) <= sum(int(types[t]) for t in ts) for key, ts in _AUGMENTED_FIELDS)
+    return _augment_counts_safe([blob.count(key) for key, _ in _AUGMENTED_FIELDS], types)
+
+
+def _augment_counts_safe(counts, types) -> bool:
+    """_augment_safe from the bytes.count of every _AUGMENTED_FIELDS key (in that order), e.g. counted on the device"""
+    return all(int(c) <= sum(int(types[t]) for t in ts) for c, (_, ts) in zip(counts, _AUGMENTED_FIELDS))
 
 
 class _GrpRun:
@@ -512,26 +529,28 @@ def _grp_run(D, device: int, with_types: bool = False) -> _GrpRun:
 
 
 def _grp_device(paths):
-    """Grp.load_gz_log_files on the device (_logio.log_device()): per chunk of files, read + gunzip on a thread pool, decode with
-    the deltas output, k_grp_logs, one copy back; the files it cannot take, in order, through the host code"""
+    """Grp.load_gz_log_files on the device (_logio.log_device()): per chunk of files, the raw bytes read on a thread pool and
+    gunzipped on the device (_logio.stage), decoded with the deltas output, k_grp_logs, one copy back; the files it cannot take,
+    in order, through the host code"""
     import torch
 
     from . import _lib
-    from .validate_logs import decode_dev
+    from .validate_logs import decode_dev_text
 
     device = _logio.log_device()
     _lib.init(device)
     out = []
     workers = min(32, os.cpu_count() or 1)
     # torch.cuda.device: the streams and allocations below belong to `device` whatever torch's current device is
-    with torch.cuda.device(device), ThreadPoolExecutor(workers) as pool:  # zlib and file reads release the GIL
-        for chunk, blobs in _logio.chunks(paths, pool, 4 * workers, _logio.read_gz, _logio.CHUNK_LOGS, _logio.CHUNK_BYTES):
+    with torch.cuda.device(device), ThreadPoolExecutor(workers) as pool:  # file reads release the GIL
+        for chunk, items in _logio.chunks(paths, pool, 4 * workers, _logio.read_gz_file, _logio.CHUNK_LOGS, _logio.CHUNK_BYTES,
+                                          _logio.text_size):
             res = [None] * len(chunk)
-            on_dev = [k for k, b in enumerate(blobs) if b is not None]  # a file that is not UTF-8 is declined by the decoder
-            if on_dev:
-                D = decode_dev([blobs[k] for k in on_dev], device, deltas=True)
+            T = _logio.stage(items, device, pool)
+            if T.files:  # a file that is not UTF-8 is declined by the decoder
+                D = decode_dev_text(T.text, T.log_off, device, deltas=True, status=T.status)
                 G = _grp_run(D, device)
-                for j, k in enumerate(on_dev):
+                for j, k in enumerate(T.files):
                     if D.accept[j]:
                         res[k] = G.grp(D, j)
             for k, path in enumerate(chunk):

@@ -6,10 +6,10 @@ IEEE semantics (0/0 = nan, x/0 = ±inf) like the Rust `as f64` divisions.
     Stat.from_dir(dir, player_name)            (every dir/**/*.json and dir/**/*.json.gz)
     python -m mortal_b200.stat DIR PLAYER_NAME (bin/stat.rs: prints the reference's report)
 
-With libmjx built and a CUDA device present, from_dir decodes the log texts on the device (k_mjai_decode with the deltas output,
-csrc/mjx_mjai.cuh) and runs Stat.from_game there for every selected seat (k_stat_logs, csrc/mjx_stat.cuh); the counters are
-summed on the device and copied back once per chunk. A file the device cannot take as it is (unreadable, not gzip, not UTF-8,
-declined by the decoder, a hora or ryukyoku without deltas for a selected seat, a first event that is not start_game, a selected
+With libmjx built and a CUDA device present, from_dir gunzips the files on the device (k_gunzip, csrc/mjx_inflate.cuh), decodes
+the log texts there (k_mjai_decode with the deltas output, csrc/mjx_mjai.cuh) and runs Stat.from_game there for every selected
+seat (k_stat_logs, csrc/mjx_stat.cuh); the counters are summed on the device and copied back once per chunk. A file the device
+cannot take as it is (unreadable, not gzip or declined by k_gunzip, not UTF-8, declined by the decoder, a hora or ryukyoku without deltas for a selected seat, a first event that is not start_game, a selected
 seat past 3) is read by the host code below, so it gives the same counters or raises the same exception. Without the library or
 a device, every file is read on the host.
 """
@@ -303,10 +303,10 @@ def _read_counters():
     return tuple(name for (name,) in _cdecl.xmacro(_cdecl.header(), "MJX_STAT_COUNTERS"))
 
 
-def _seat_mask(blob: bytes, b: int, e: int, player_name: str):
-    """the seats named player_name on a log's first event line (bytes [b, e)) as a bit mask, or None when the host must decide"""
+def _seat_mask(first: bytes, player_name: str):
+    """the seats named player_name on a log's first event line as a bit mask, or None when the host must decide"""
     try:
-        first = json.loads(blob[b:e].decode("utf-8"))
+        first = json.loads(first.decode("utf-8"))
         if first.get("type") != "start_game":
             return None
         seats = [i for i, name in enumerate(first.get("names", [])) if name == player_name]
@@ -324,14 +324,14 @@ def _chunks(paths, pool, step: int):
 
 
 def _device_from_dir(paths, player_name: str, device: int | None = None) -> Stat:
-    """from_dir on the device (default: _stat_device()): per chunk of files, read + gunzip on a thread pool, decode with the deltas
-    output, k_stat_logs over the seats of every log, the counters summed on the device and copied back once; the rest of the
-    chunk's files, in glob order, through _host_log_stat"""
+    """from_dir on the device (default: _stat_device()): per chunk of files, the raw bytes read on a thread pool and gunzipped on
+    the device (_logio.stage), decoded with the deltas output, k_stat_logs over the seats of every log, the counters summed on the
+    device and copied back once; the rest of the chunk's files, in glob order, through _host_log_stat"""
     import numpy as np
     import torch
 
     from . import _lib
-    from .validate_logs import decode_dev
+    from .validate_logs import decode_dev_text
 
     device = _stat_device() if device is None else device
     _lib.init(device)
@@ -342,21 +342,23 @@ def _device_from_dir(paths, player_name: str, device: int | None = None) -> Stat
     host_total = Stat()
     workers = min(32, os.cpu_count() or 1)
     # torch.cuda.device: the streams and allocations below belong to `device` whatever torch's current device is
-    with torch.cuda.device(device), ThreadPoolExecutor(workers) as pool:  # zlib and file reads release the GIL
-        for chunk, blobs in _chunks(paths, pool, 4 * workers):
-            on_dev = [k for k, b in enumerate(blobs) if b is not None]
-            host = [k for k, b in enumerate(blobs) if b is None]
-            if on_dev:
-                D = decode_dev([blobs[k] for k in on_dev], device, deltas=True)
-                seats = np.zeros(len(on_dev), dtype=np.uint8)
+    with torch.cuda.device(device), ThreadPoolExecutor(workers) as pool:  # file reads release the GIL
+        for chunk, items in _logio.chunks(paths, pool, 4 * workers, _logio.read_file, CHUNK_LOGS, CHUNK_BYTES, _logio.text_size):
+            T = _logio.stage(items, device, pool)
+            host = [k for k in range(len(chunk)) if k not in set(T.files)]
+            if T.files:
+                D = decode_dev_text(T.text, T.log_off, device, deltas=True, status=T.status)
+                n = len(T.files)
+                acc = np.nonzero(D.accept)[0]
+                firsts = dict(zip(acc, _logio.spans(T.text, T.log_off, acc, D.counts[acc, 4], D.counts[acc, 5], device)))
+                seats = np.zeros(n, dtype=np.uint8)
                 counted = []
-                for j, k in enumerate(on_dev):
-                    m = _seat_mask(blobs[k], int(D.counts[j, 4]), int(D.counts[j, 5]), player_name) if D.accept[j] else None
+                for j, k in enumerate(T.files):
+                    m = _seat_mask(firsts[j], player_name) if D.accept[j] else None
                     if m is None:
                         host.append(k)
                     else:
                         seats[j] = m; counted.append(j)
-                n = len(on_dev)
                 out = torch.empty((n, len(names)), dtype=torch.int64, device=dev)
                 status = torch.empty(n, dtype=torch.int32, device=dev)
                 d_seats = torch.from_numpy(seats).to(dev)
@@ -370,7 +372,7 @@ def _device_from_dir(paths, player_name: str, device: int | None = None) -> Stat
                 for name, v in zip(names, res[:len(names)]):
                     total[name] += int(v)
                 st = res[len(names):]
-                host += [on_dev[j] for j in counted if st[j] != 0]
+                host += [T.files[j] for j in counted if st[j] != 0]
             for k in sorted(host):
                 host_total = host_total + _host_log_stat(chunk[k], player_name)
     return Stat(**total) + host_total

@@ -4,7 +4,8 @@
     python -m mortal_b200.validate_logs DIR       (every DIR/**/*.json and DIR/**/*.json.gz, in sorted order)
 
 The log text is decoded into event words on the device (k_mjai_decode, csrc/mjx_mjai.cuh), and the words go straight to the
-k_validate_logs kernel (csrc/mjx_validate.cuh), which runs the rule checks and the state updates. A log the device decoder
+k_validate_logs kernel (csrc/mjx_validate.cuh), which runs the rule checks and the state updates. The CLI gunzips the .json.gz
+files on the device too (k_gunzip, csrc/mjx_inflate.cuh); a file k_gunzip declines is read on the host. A log the device decoder
 declines (anything it cannot show Python's json reads the same way, and every log that fails to parse) is decoded on the host
 by encode_log (json.loads + dataset_codec.check_event, reported as PARSE) exactly as before; the verdicts do not depend on the
 path. There is no CPU path: without a CUDA device validate_logs raises.
@@ -121,25 +122,38 @@ class DecodedLogs:
 
 
 def decode_dev(blobs, device: int = 0, augment: bool = False, deltas: bool = False) -> DecodedLogs:
-    """UTF-8 log texts (bytes) -> DecodedLogs, decoded on `device` (csrc/mjx_mjai.cuh); the one device-to-host copy is the counts.
-    `deltas` also fills the per-event deltas arrays (mjx_mjai_fill_deltas_dev); the other arrays are the same either way."""
+    """UTF-8 log texts (bytes) -> DecodedLogs, decoded on `device` (csrc/mjx_mjai.cuh): the texts copied once into pinned memory
+    and once to the device, then decode_dev_text"""
     import torch
 
-    L = _lib.load()
     n = len(blobs)
-    dev = torch.device("cuda", device)
-    st = torch.cuda.current_stream(dev).cuda_stream
     log_off = np.zeros(n + 1, dtype=np.int64)
     np.cumsum([len(b) for b in blobs], out=log_off[1:])
     staged = torch.empty(max(int(log_off[-1]), 1), dtype=torch.uint8, pin_memory=True)  # the texts copied once, into pinned memory
     view = staged.numpy()
     for b, o in zip(blobs, log_off):
         view[o:o + len(b)] = np.frombuffer(b, dtype=np.uint8)
-    text = staged.to(dev, non_blocking=True)  # `staged` lives until the counts' copy below has synchronised the stream
-    d_off = torch.from_numpy(log_off).to(dev)
+    text = staged.to(torch.device("cuda", device), non_blocking=True)  # `staged` lives until the counts' copy has synchronised
+    return decode_dev_text(text, log_off, device, augment, deltas)
+
+
+def decode_dev_text(text, log_off, device: int = 0, augment: bool = False, deltas: bool = False, status=None) -> DecodedLogs:
+    """The log texts text[log_off[i], log_off[i + 1]) (a uint8 tensor on `device`; log_off int64 [n + 1] on the host) ->
+    DecodedLogs; the one device-to-host copy is the counts. `deltas` also fills the per-event deltas arrays
+    (mjx_mjai_fill_deltas_dev); the other arrays are the same either way. `status` (int32 [n] on the device, e.g.
+    _logio.DeviceText.status) declines every log whose entry is not 0, as the decoder declines a log."""
+    import torch
+
+    L = _lib.load()
+    n = len(log_off) - 1
+    dev = torch.device("cuda", device)
+    st = torch.cuda.current_stream(dev).cuda_stream
+    d_off = torch.from_numpy(np.ascontiguousarray(log_off, dtype=np.int64)).to(dev)
     d_counts = torch.empty((n, 6), dtype=torch.int32, device=dev)
     _lib.check(L.mjx_mjai_count_dev(n, text.data_ptr(), int(log_off[-1]), d_off.data_ptr(), int(augment), d_counts.data_ptr(), st),
                "mjx_mjai_count_dev")
+    if status is not None:  # before the copy back: the fill pass reads these counts too
+        d_counts.masked_fill_((status != 0).unsqueeze(1), 0)
     counts = d_counts.cpu().numpy()
     accept = counts[:, 0] != 0
     excl = lambda x: (np.cumsum(x) - x).astype(np.int32)
@@ -186,10 +200,7 @@ def _event_lines(text: str) -> _Lines:
 def _validate(texts, device: int = 0):
     """-> ([Verdict | None], per log the EncodedLog / line list message() reads, or None for a valid log decoded on the device).
     Logs are decoded on the device; those it declines go through encode_log, as do texts that are not valid UTF-8."""
-    import torch
-
     _lib.init(device)  # no CUDA device: raises before any work, whatever the logs
-    L = _lib.load()
     out, enc = [None] * len(texts), [None] * len(texts)
     blobs, idx, host = [], [], []  # host: the logs encode_log decodes
     for i, t in enumerate(texts):
@@ -201,29 +212,77 @@ def _validate(texts, device: int = 0):
         except UnicodeEncodeError:  # lone surrogates: not UTF-8, so the host decides
             host.append(i)
     if blobs:
-        D = decode_dev(blobs, device)
-        n = len(blobs)
-        dev = torch.device("cuda", device)
-        verd = torch.empty((n, 4), dtype=torch.int32, device=dev)
-        ptr = lambda t: t.data_ptr() if t.numel() else None
-        _lib.check(L.mjx_validate_logs_dev(n, ptr(D.hdr), D.offs[0].data_ptr(), D.offs[1].data_ptr(), D.hdr.numel(), ptr(D.kyoku),
-                                           D.offs[2].data_ptr(), D.kyoku.numel(), ptr(D.hora), D.offs[3].data_ptr(), D.hora.numel(),
-                                           verd.data_ptr(), torch.cuda.current_stream(dev).cuda_stream), "mjx_validate_logs_dev")
-        rows = verd.cpu().numpy()
-        bad = np.nonzero(D.accept & (rows[:, 0] != 0))[0]
-        ev = rows[bad, 2].astype(np.int64)
-        inside = (ev > 0) & (ev <= D.ev_cnt[bad])
-        lines = np.array(ev)
-        if inside.any():  # the line of the failing event, from the device line array
-            at = torch.from_numpy(D.ev_off[bad][inside].astype(np.int64) + ev[inside] - 1).to(dev)
-            lines[inside] = D.lines[at].cpu().numpy()
-        for k, b in enumerate(bad):
-            status, reason, _, seat = (int(x) for x in rows[b])
-            out[idx[b]] = Verdict(STATUSES[status], REASONS[reason], int(lines[k]), seat)
-            enc[idx[b]] = _event_lines(texts[idx[b]])
-        host += [idx[k] for k in np.nonzero(~D.accept)[0]]
+        host += _device_verdicts(decode_dev(blobs, device), idx, out, enc, texts.__getitem__, device)
+    _host_verdicts(sorted(host), out, enc, texts.__getitem__, device)
+    return out, enc
+
+
+def _validate_files(paths, items, pool=None, device: int = 0):
+    """_validate over files: items = _logio.read_file of every path. The .gz files are gunzipped on the device and the plain
+    ones read as text on the host and copied into the same buffer; a file the device cannot take, or whose log it declines, is
+    read on the host by _read (as is a failing log's text, for its message)."""
+    from . import _logio
+
+    _lib.init(device)
+    n = len(paths)
+    out, enc = [None] * n, [None] * n
+    texts = {}
+
+    def text_of(i):
+        if i not in texts:
+            texts[i] = _read(paths[i])
+        return texts[i]
+
+    staged = list(items)
+    for i, (raw, gz) in enumerate(staged):
+        if not gz:  # a plain file: the text the host reads, as UTF-8
+            t = text_of(i)
+            staged[i] = (t.encode("utf-8") if isinstance(t, str) else None, False)
+    T = _logio.stage(staged, device, pool)
+    host = [i for i in range(n) if i not in set(T.files)]
+    if T.files:
+        D = decode_dev_text(T.text, T.log_off, device, status=T.status)
+        host += _device_verdicts(D, T.files, out, enc, text_of, device)
+    host.sort()  # read on the host in file order, so a file that raises does so where the host path's read raises
     for i in host:
-        enc[i] = encode_log(texts[i])
+        if isinstance(text_of(i), Verdict):
+            out[i] = enc[i] = text_of(i)
+    _host_verdicts([i for i in host if out[i] is None], out, enc, text_of, device)
+    return out, enc
+
+
+def _device_verdicts(D, idx, out, enc, text_of, device: int):
+    """the verdicts of the logs D decoded (log j is item idx[j]) into out / enc (a failing log's event lines from text_of(item));
+    returns the items D declined"""
+    import torch
+
+    L = _lib.load()
+    n = len(idx)
+    dev = torch.device("cuda", device)
+    verd = torch.empty((n, 4), dtype=torch.int32, device=dev)
+    ptr = lambda t: t.data_ptr() if t.numel() else None
+    _lib.check(L.mjx_validate_logs_dev(n, ptr(D.hdr), D.offs[0].data_ptr(), D.offs[1].data_ptr(), D.hdr.numel(), ptr(D.kyoku),
+                                       D.offs[2].data_ptr(), D.kyoku.numel(), ptr(D.hora), D.offs[3].data_ptr(), D.hora.numel(),
+                                       verd.data_ptr(), torch.cuda.current_stream(dev).cuda_stream), "mjx_validate_logs_dev")
+    rows = verd.cpu().numpy()
+    bad = np.nonzero(D.accept & (rows[:, 0] != 0))[0]
+    ev = rows[bad, 2].astype(np.int64)
+    inside = (ev > 0) & (ev <= D.ev_cnt[bad])
+    lines = np.array(ev)
+    if inside.any():  # the line of the failing event, from the device line array
+        at = torch.from_numpy(D.ev_off[bad][inside].astype(np.int64) + ev[inside] - 1).to(dev)
+        lines[inside] = D.lines[at].cpu().numpy()
+    for k, b in enumerate(bad):
+        status, reason, _, seat = (int(x) for x in rows[b])
+        out[idx[b]] = Verdict(STATUSES[status], REASONS[reason], int(lines[k]), seat)
+        enc[idx[b]] = _event_lines(text_of(idx[b]))
+    return [idx[k] for k in np.nonzero(~D.accept)[0]]
+
+
+def _host_verdicts(host, out, enc, text_of, device: int):
+    """encode_log, then one mjx_validate_logs launch, over the items `host` (texts from text_of(item))"""
+    for i in host:
+        enc[i] = encode_log(text_of(i))
         if isinstance(enc[i], Verdict):
             out[i] = enc[i]
     replay = [i for i in host if isinstance(enc[i], EncodedLog)]
@@ -231,7 +290,6 @@ def _validate(texts, device: int = 0):
         rows = run_packed(pack([enc[i] for i in replay]), device)
         for i, r in zip(replay, rows):
             out[i] = to_verdict(r, enc[i])
-    return out, enc
 
 
 def validate_logs(texts, device: int = 0):
@@ -288,10 +346,13 @@ def main(argv=None) -> int:
     d = argv[0]
     paths = sorted(set(glob.glob(os.path.join(d, "**", "*.json"), recursive=True))
                    | set(glob.glob(os.path.join(d, "**", "*.json.gz"), recursive=True)))
-    with ThreadPoolExecutor(min(32, os.cpu_count() or 1)) as pool:  # zlib and file reads release the GIL
-        for lo in range(0, len(paths), CHUNK_LOGS):
-            chunk = paths[lo:lo + CHUNK_LOGS]
-            verdicts, enc = _validate(list(pool.map(_read, chunk)))
+    from . import _logio
+
+    workers = min(32, os.cpu_count() or 1)
+    with ThreadPoolExecutor(workers) as pool:  # file reads release the GIL
+        for chunk, items in _logio.chunks(paths, pool, 4 * workers, _logio.read_file, CHUNK_LOGS, _logio.CHUNK_BYTES,
+                                          _logio.text_size):
+            verdicts, enc = _validate_files(chunk, items, pool)
             for path, v, e in zip(chunk, verdicts, enc):
                 if v is not None:
                     print(f"\nerror in log {path}\n{message(v, e)}", flush=True)
