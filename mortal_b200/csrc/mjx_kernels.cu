@@ -8,9 +8,11 @@
 #include <vector>
 
 #include "../../include/mjx.h"
+#include "../../include/mjx_review.h"
 #include "mjx_sp.cuh"
 #include "mjx_policy.cuh"
 #include "mjx_replay.cuh"
+#include "mjx_review.cuh"
 #include "mjx_validate.cuh"
 #include "mjx_mjai.cuh"
 #include "mjx_inflate.cuh"
@@ -104,7 +106,59 @@ __global__ void __launch_bounds__(VIEW_WARPS * 32) k_replay_viewpoints(TableStat
     const int job = blockIdx.x * VIEW_WARPS + warp;
     if (job >= n_jobs) return;
     const int mask = replay_hidden_seats(R, job, n_hdr, n_kyoku, lane);
-    if (lane == 0) replay_mark_viewpoint(tabs + job, R.player[job], mask);
+    if (lane == 0) replay_mark_viewpoint(tabs + job, R.player[job], mask, R.review != 0);
+}
+
+// Review (csrc/mjx_review.cuh): one warp = one decision of the step (its main row), with the record still at the decision.
+__global__ void __launch_bounds__(STEP_WARPS * 32) k_review_react(EnvView V, ReplayView R, Tables T, int n_rows, const i64* actions,
+                                                                  const float* q, const u8* greedy, int guard, ReviewOut O) {
+    __shared__ WarpScratch s_scratch[STEP_WARPS];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int row = blockIdx.x * STEP_WARPS + warp;
+    if (row >= n_rows || (V.row_seat[row] & 4)) return;  // a kan-select row belongs to the decision row before it
+    Ctx c;
+    c.S = V.tables + V.row_table[row];
+    c.W = &s_scratch[warp];
+    c.T = T;
+    c.lane = lane;
+    c.df = s_scratch[warp].dora_factor;
+    recompute_dora_factor(c);
+    review_react_row(c, V, R, row, n_rows, actions, q, greedy, guard != 0, O);
+}
+
+// One warp = one job; the lines go 32 at a time, one per lane, placed by a warp prefix sum of their sizes.
+template <bool FILL>
+__global__ void __launch_bounds__(MW_WARPS * 32) k_review_render(RvView V) {
+    const int lane = threadIdx.x & 31;
+    const int j = blockIdx.x * MW_WARPS + (threadIdx.x >> 5);
+    if (j >= V.n_jobs) return;
+    if (V.skip && V.skip[j]) {
+        if (!FILL && lane == 0) V.bytes[j] = 0;
+        return;
+    }
+    const int n = V.ev_cnt[j];
+    long long total = 0;
+    for (int base = 0; base < n; base += 32) {
+        const int e = base + lane;
+        long long size = 0;
+        if (e < n) {
+            MwOut o{nullptr, 0, 0};
+            rv_line(o, V, j, e);
+            size = o.n;
+        }
+        long long incl = size;
+        for (int d = 1; d < 32; d <<= 1) {
+            const long long y = __shfl_up_sync(~0u, incl, d);
+            if (lane >= d) incl += y;
+        }
+        if (FILL && e < n) {
+            const long long at = V.off[j] + total + incl - size;
+            MwOut o{V.out + at, 0, V.out_cap - at};
+            rv_line(o, V, j, e);
+        }
+        total += __shfl_sync(~0u, incl, 31);
+    }
+    if (!FILL && lane == 0) V.bytes[j] = total;
 }
 
 // Log validation (csrc/mjx_validate.cuh): one warp = one whole log. The record is initialised in shared memory and never
@@ -625,13 +679,7 @@ __global__ void __launch_bounds__(STEP_WARPS * 32) k_state_query(EnvView V, Tabl
         i32 err = 0;
         const bool okd = decode_action(c.S, p, args[0], args[1], r, &err);
         if (lane == 0) {
-            u64 w = 0;
-            if (okd) {
-                const int ty = r.type == R_DAHAI ? LOG_DAHAI : r.type == R_CHI ? LOG_CHI : r.type == R_PON ? LOG_PON :
-                               r.type == R_DAIMINKAN ? LOG_DAIMINKAN : r.type == R_KAKAN ? LOG_KAKAN : r.type == R_ANKAN ? LOG_ANKAN :
-                               r.type == R_REACH ? LOG_REACH : r.type == R_HORA ? LOG_HORA : r.type == R_RYUKYOKU ? LOG_RYUKYOKU : 0;
-                w = log_word(ty, r.actor, r.target, r.pai, r.tsumogiri, 0, r.consumed[0], r.consumed[1], r.consumed[2], r.consumed[3], 0);
-            }
+            const u64 w = okd ? reaction_word(r) : 0;
             out[0] = (i32)(u32)w; out[1] = (i32)(u32)(w >> 32); out[2] = okd ? 0 : (err ? err : ERR_ILLEGAL_ACTION);
         }
     }
@@ -2064,6 +2112,73 @@ int mjx_env_replay_step(mjx_env* env, void* stream) {
     env->first = false;
     return MJX_OK;
 }
+int mjx_env_replay_review(mjx_env* env, void* stream) {
+    if (!env || !env->replay) return fail(MJX_ERR_ARG, "mjx_env_replay_review: not a replay env");
+    if (env->R.trust_seed || env->viewpoints)
+        return fail(MJX_ERR_ARG, "mjx_env_replay_review: not with mjx_env_replay_trust_seeds or mjx_env_replay_viewpoints");
+    if (!env->first) return fail(MJX_ERR_STATE, "mjx_env_replay_review: must be called before the first mjx_env_replay_step");
+    env->R.review = 1;
+    k_replay_viewpoints<<<(env->n_tables + VIEW_WARPS - 1) / VIEW_WARPS, VIEW_WARPS * 32, 0, (cudaStream_t)stream>>>(
+        env->V.tables, env->R, env->n_tables, env->r_n_hdr, env->r_n_kyoku);
+    CU(cudaGetLastError());
+    env->launches += 1;
+    env->viewpoints = true;
+    return MJX_OK;
+}
+
+int mjx_review_react_dev(mjx_env* env, int n_rows, const int64_t* actions, const float* q, const uint8_t* greedy, int agari_guard,
+                         int32_t* info, uint64_t* mask, float* q_out, int64_t* i64s, uint64_t* word, void* stream) {
+    if (!env || !env->replay || !env->R.review || n_rows < 0 || n_rows > env->row_cap || !actions || !q || !greedy || !info || !mask ||
+        !q_out || !i64s || !word)
+        return fail(MJX_ERR_ARG, "mjx_review_react_dev: bad arguments");
+    if (n_rows == 0) return MJX_OK;
+    const ReviewOut O{info, mask, q_out, i64s, word};
+    k_review_react<<<(n_rows + STEP_WARPS - 1) / STEP_WARPS, STEP_WARPS * 32, 0, (cudaStream_t)stream>>>(
+        env->V, env->R, g_T, n_rows, actions, q, greedy, agari_guard, O);
+    CU(cudaGetLastError());
+    env->launches += 1;
+    return MJX_OK;
+}
+
+static bool rv_view(RvView& V, int n_jobs, const int32_t* ev_cnt, const int64_t* rec_off, long long n_rec, const int32_t* rec_event,
+                    const uint8_t* rec_kan, const uint64_t* rec_word, const int32_t* rec_info, const uint64_t* rec_mask,
+                    const float* rec_q, const int64_t* rec_i64, const uint8_t* skip) {
+    if (n_jobs <= 0 || !ev_cnt || !rec_off || n_rec < 0 || (n_rec > 0 && (!rec_event || !rec_kan || !rec_word || !rec_info ||
+                                                                          !rec_mask || !rec_q || !rec_i64)))
+        return false;
+    V = RvView{};
+    V.ev_cnt = ev_cnt; V.rec_off = rec_off; V.rec_event = rec_event; V.rec_kan = rec_kan; V.rec_word = rec_word; V.skip = skip;
+    V.M.rec_info = rec_info; V.M.rec_mask = rec_mask; V.M.rec_q = rec_q; V.M.rec_i64 = rec_i64; V.M.n_rec = n_rec;
+    V.n_jobs = n_jobs;
+    return true;
+}
+
+int mjx_review_render_count_dev(int n_jobs, const int32_t* ev_cnt, const int64_t* rec_off, long long n_rec, const int32_t* rec_event,
+                                const uint8_t* rec_kan, const uint64_t* rec_word, const int32_t* rec_info, const uint64_t* rec_mask,
+                                const float* rec_q, const int64_t* rec_i64, const uint8_t* skip, int64_t* bytes, void* stream) {
+    RvView V;
+    if (!rv_view(V, n_jobs, ev_cnt, rec_off, n_rec, rec_event, rec_kan, rec_word, rec_info, rec_mask, rec_q, rec_i64, skip) || !bytes)
+        return fail(MJX_ERR_ARG, "mjx_review_render_count_dev: bad arguments");
+    V.bytes = bytes;
+    k_review_render<false><<<(n_jobs + MW_WARPS - 1) / MW_WARPS, MW_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
+int mjx_review_render_fill_dev(int n_jobs, const int32_t* ev_cnt, const int64_t* rec_off, long long n_rec, const int32_t* rec_event,
+                               const uint8_t* rec_kan, const uint64_t* rec_word, const int32_t* rec_info, const uint64_t* rec_mask,
+                               const float* rec_q, const int64_t* rec_i64, const uint8_t* skip, const int64_t* off, char* out,
+                               long long out_cap, void* stream) {
+    RvView V;
+    if (!rv_view(V, n_jobs, ev_cnt, rec_off, n_rec, rec_event, rec_kan, rec_word, rec_info, rec_mask, rec_q, rec_i64, skip) || !off ||
+        out_cap < 0 || (out_cap > 0 && !out))
+        return fail(MJX_ERR_ARG, "mjx_review_render_fill_dev: bad arguments");
+    V.off = off; V.out = out; V.out_cap = out_cap;
+    k_review_render<true><<<(n_jobs + MW_WARPS - 1) / MW_WARPS, MW_WARPS * 32, 0, (cudaStream_t)stream>>>(V);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+
 int64_t* mjx_env_row_label(mjx_env* env) { return env && env->replay ? (int64_t*)env->R.row_label : nullptr; }
 uint8_t* mjx_env_row_meta(mjx_env* env) { return env && env->replay ? env->R.row_meta : nullptr; }
 

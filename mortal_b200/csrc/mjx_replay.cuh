@@ -30,6 +30,8 @@ struct ReplayView {
     i32 always_include_kan_select;
     i32 trust_seed;     // the jobs carry their game's seed (TableState.nonce / key): regenerate every kyoku's wall from it
                         // (dataset/invisible.rs:35-66), which the invisible observation needs; else hidden tiles stay unknown
+    i32 review;         // review mode (mjx_env_replay_review, csrc/mjx_review.cuh): every event is applied and the job stops
+                        // wherever its seat can act, as mjai.Bot with quick eval off decides; labels where the log shows one
 };
 
 MJX_D int lw_type(u64 w) { return (int)(w & 0xFF); }
@@ -172,21 +174,25 @@ MJX_DM int replay_hidden_seats(const ReplayView& R, int job, long long n_hdr, lo
 
 // The job's record after the scan: a log that hides a seat is replayed from the player's own PlayerState (viewer1 = player + 1;
 // dataset/gameplay.rs:240-335 with oracle = false runs only that state), and fails at once with ERR_HIDDEN_OWN_TILE when it hides
-// the player's own tiles. A full-information log (mask 0) and an unmarked job (-1) are left untouched.
-MJX_D void replay_mark_viewpoint(TableState* S, int player, int mask) {
-    if (mask <= 0 || player > 3) return;
+// the player's own tiles. A full-information log (mask 0) is left untouched unless `every_log` (review mode: the Bot's state is a
+// PlayerState whatever the log shows); an unmarked job (-1) always is.
+MJX_D void replay_mark_viewpoint(TableState* S, int player, int mask, bool every_log = false) {
+    if (mask < 0 || (mask == 0 && !every_log) || player > 3) return;
     S->viewer1 = (u8)(player + 1);
     if (((mask >> player) & 1) && S->err == 0) S->err = ERR_HIDDEN_OWN_TILE;
 }
 
-// Advance one job to its next logged decision. Returns true while the job still has events to process.
+// Advance one job to its next logged decision (review mode: to its seat's next event with CAN_ACT). Returns true while the job
+// still has events to process.
 MJX_DN bool replay_table(Ctx& c, EnvView& V, const ReplayView& R, int job) {
     TableState* S = c.S;
     if (!(S->gflags & GF_ALIVE)) return false;
     recompute_dora_factor(c);
     const int n = R.ev_cnt[job], p = R.player[job];
     const u64* ev = R.hdr + R.ev_off[job];
-    for (int w = R.pos[job]; w + 4 <= n; w++) {  // gameplay.rs:279-283: windows of four events
+    const int end = R.review ? n : n - 3;  // gameplay.rs:279-283: windows of four events (w + 4 <= n); review: every event
+    int w = R.pos[job];
+    for (; w < end; w++) {
         const u64 cur = ev[w];
         if (lw_type(cur) == LOG_END_KYOKU) { MJX_L0(R.ky_idx[job] += 1); }
         replay_apply(c, R, job, cur);
@@ -195,9 +201,12 @@ MJX_DN bool replay_table(Ctx& c, EnvView& V, const ReplayView& R, int job) {
         const SeatPrivate& P = S->priv[p];
         const u16 cans = P.cans;
         if (!(cans & CAN_ACT)) continue;
-        const int t1 = lw_type(ev[w + 1]);
-        const u64 next = (t1 == LOG_REACH_ACCEPTED || t1 == LOG_DORA) ? ev[w + 2] : ev[w + 1];
+        // the look-ahead stops at the end of the log (type 0 = no event); inside the four-event window it never reaches it
+        const int t1 = w + 1 < n ? lw_type(ev[w + 1]) : 0;
+        const int wn = (t1 == LOG_REACH_ACCEPTED || t1 == LOG_DORA) ? w + 2 : w + 1;
+        const u64 next = wn < n ? ev[wn] : 0;
         const int tn = lw_type(next);
+        const bool kan_always = R.always_include_kan_select || R.review;
         int label = -1, kan_select = -1;
         bool catch_all = false;
         switch (tn) {  // gameplay.rs:349-421
@@ -215,11 +224,11 @@ MJX_DN bool replay_table(Ctx& c, EnvView& V, const ReplayView& R, int job) {
                 else catch_all = true;
                 break;
             case LOG_KAKAN:
-                if (R.always_include_kan_select || mjx_popcll(P.kakan_cand) > 1) kan_select = deaka(lw_pai(next));
+                if (kan_always || mjx_popcll(P.kakan_cand) > 1) kan_select = deaka(lw_pai(next));
                 label = 42;
                 break;
             case LOG_ANKAN:
-                if (R.always_include_kan_select || mjx_popcll(P.ankan_cand) > 1) kan_select = deaka(lw_c(next, 0));
+                if (kan_always || mjx_popcll(P.ankan_cand) > 1) kan_select = deaka(lw_c(next, 0));
                 label = 42;
                 break;
             case LOG_RYUKYOKU: if (cans & CAN_RYUKYOKU) label = 44; else catch_all = true; break;
@@ -228,7 +237,7 @@ MJX_DN bool replay_table(Ctx& c, EnvView& V, const ReplayView& R, int job) {
         if (catch_all) {
             const bool has_any_ron = t1 == LOG_HORA;
             if (has_any_ron)
-                for (int k = w + 1; k < w + 4; k++) {
+                for (int k = w + 1; k < w + 4 && k < n; k++) {
                     const int tk = lw_type(ev[k]);
                     if (tk == LOG_END_KYOKU) break;
                     if (tk == LOG_HORA && lw_actor(ev[k]) == p) { label = 43; break; }
@@ -238,9 +247,11 @@ MJX_DN bool replay_table(Ctx& c, EnvView& V, const ReplayView& R, int job) {
                 if ((can_chi && tn == LOG_TSUMO) || ((cans & (CAN_PON | CAN_DAIMINKAN | CAN_RON_AGARI)) && !has_any_ron)) label = 45;
             }
         }
-        if (label < 0) continue;
-        // gameplay.rs:425-447 add_entry: the decision row, then the kan-select row
-        const int n_rows = kan_select >= 0 ? 2 : 1;
+        if (label < 0 && !R.review) continue;
+        // gameplay.rs:425-447 add_entry: the decision row, then the kan-select row; review mode: the kan-select row whenever an
+        // ankan or kakan is possible (agent/mortal.rs set_scene with quick eval off), labelled only when the log shows the kan
+        const bool kan_row = R.review ? (cans & (CAN_ANKAN | CAN_KAKAN)) != 0 : kan_select >= 0;
+        const int n_rows = kan_row ? 2 : 1;
         const int base = alloc_rows(c, V, n_rows);
         if (base + n_rows > V.row_cap) { set_err(c, ERR_ROW_OVERFLOW); break; }
         const u64 discards = (cans & CAN_DISCARD) ? discard_candidates(c, p) : 0;
@@ -257,7 +268,8 @@ MJX_DN bool replay_table(Ctx& c, EnvView& V, const ReplayView& R, int job) {
         MJX_SYNCWARP();
         return true;
     }
-    MJX_L0(R.pos[job] = n; S->gflags &= (u8)~GF_ALIVE; V.done[job] = 1; V.err[job] = S->err);
+    // review mode: steps = the event the job stopped at (the failing one, or n)
+    MJX_L0(R.pos[job] = n; S->gflags &= (u8)~GF_ALIVE; V.done[job] = 1; V.err[job] = S->err; if (R.review) V.steps[job] = w);
     MJX_SYNCWARP();
     return false;
 }

@@ -1294,6 +1294,14 @@ MJX_DN bool decode_action(const TableState* S, int seat, int action, int kan_act
     return true;
 }
 
+// a decoded reaction as an event word (log_word; type 0 = none): what libriichi.state.reaction_from_word reads back
+MJX_D u64 reaction_word(const Reaction& r) {
+    const int ty = r.type == R_DAHAI ? LOG_DAHAI : r.type == R_CHI ? LOG_CHI : r.type == R_PON ? LOG_PON :
+                   r.type == R_DAIMINKAN ? LOG_DAIMINKAN : r.type == R_KAKAN ? LOG_KAKAN : r.type == R_ANKAN ? LOG_ANKAN :
+                   r.type == R_REACH ? LOG_REACH : r.type == R_HORA ? LOG_HORA : r.type == R_RYUKYOKU ? LOG_RYUKYOKU : 0;
+    return log_word(ty, r.actor, r.target, r.pai, r.tsumogiri, 0, r.consumed[0], r.consumed[1], r.consumed[2], r.consumed[3], 0);
+}
+
 // ================================================================ table step (commit + poll + emit)
 // Device-resident buffers of one environment. Plain pointers only: this struct is also what
 // include/mjx.h hands out piecewise through the C ABI.
