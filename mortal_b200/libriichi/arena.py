@@ -20,6 +20,8 @@ import numpy as np
 from ..engine import HostProtocolEngine
 from ..env import BatchEnv
 
+AKOCHAN_UNSUPPORTED = "akochan subprocess agents are out of scope (SURVEY.md §2.1 row 5)"
+
 
 def _adapt(engine):
     if hasattr(engine, "react_device"):
@@ -537,7 +539,7 @@ class _Arena:
                 pool.shutdown(wait=True)
 
     def ako_vs_py(self, *a, **k):
-        raise NotImplementedError("akochan subprocess agents are out of scope (SURVEY.md §2.1 row 5)")
+        raise NotImplementedError(AKOCHAN_UNSUPPORTED)
 
     py_vs_ako = ako_vs_py
 

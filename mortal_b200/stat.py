@@ -4,6 +4,7 @@ integer attributes with the reference's names; every derived quantity is a prope
 IEEE semantics (0/0 = nan, x/0 = ±inf) like the Rust `as f64` divisions.
 
     Stat.from_dir(dir, player_name)            (every dir/**/*.json and dir/**/*.json.gz)
+    Stat.from_games(games, player_name, idx)   (the written logs of a selfplay.SelfPlayGames, counted without the logs)
     python -m mortal_b200.stat DIR PLAYER_NAME (bin/stat.rs: prints the reference's report)
 
 With libmjx built and a CUDA device present, from_dir gunzips the files on the device (k_gunzip, csrc/mjx_inflate.cuh), decodes
@@ -211,6 +212,35 @@ class Stat:
             total = total + _host_log_stat(path, player_name)
         return total
 
+    @staticmethod
+    def from_games(games, player_name: str, idx=None) -> "Stat":
+        """from_dir over the written logs of self-play games idx (default all) of a selfplay.SelfPlayGames, without the logs: every
+        seat whose name is player_name counts (a champion at three seats counts three times). Words on a CUDA device are converted
+        there (selfplay.decode_games) and counted by k_stat_logs, the counters summed on the device and copied back once; a game
+        with a non-zero kernel status, and every game whose words are not on a CUDA device, is decoded on the host
+        (mjai_log.decode_events between its start_game and an end_game) and counted by from_game. Corrupt or overflowed words
+        raise decode_games' RuntimeError, which names the game and its seed."""
+        import numpy as np
+
+        idx = list(range(len(games))) if idx is None else [int(i) for i in idx]
+        masks = [sum(1 << s for s, name in enumerate(games.names[g]) if name == player_name) for g in idx]
+        if not idx:
+            return Stat()
+        if games.words.device.type != "cuda":
+            return _host_games_stat(games, list(zip(idx, masks)))
+        import torch
+
+        from . import _lib
+        from .selfplay import decode_games
+
+        dev = games.words.device
+        with torch.cuda.device(dev):
+            _lib.init(dev.index)
+            D = decode_games(games, idx)
+            sums, status = _stat_logs_dev(_lib.load(), D, np.array(masks, dtype=np.uint8), dev, _read_counters())
+        host = [(g, m) for g, m, st in zip(idx, masks, status) if st != 0]
+        return Stat(**sums) + _host_games_stat(games, host)
+
     def __repr__(self):
         return "Stat(" + ", ".join(f"{c}={getattr(self, c)}" for c in COUNTERS) + ")"
 
@@ -359,23 +389,65 @@ def _device_from_dir(paths, player_name: str, device: int | None = None) -> Stat
                         host.append(k)
                     else:
                         seats[j] = m; counted.append(j)
-                out = torch.empty((n, len(names)), dtype=torch.int64, device=dev)
-                status = torch.empty(n, dtype=torch.int32, device=dev)
-                d_seats = torch.from_numpy(seats).to(dev)
-                ptr = lambda t: t.data_ptr() if t.numel() else None
-                _lib.check(L.mjx_stat_logs_dev(n, ptr(D.hdr), D.offs[0].data_ptr(), D.offs[1].data_ptr(), D.hdr.numel(),
-                                               ptr(D.kyoku), D.offs[2].data_ptr(), D.kyoku.numel(), ptr(D.deltas), ptr(D.has_deltas),
-                                               d_seats.data_ptr(), out.data_ptr(), status.data_ptr(),
-                                               torch.cuda.current_stream(dev).cuda_stream), "mjx_stat_logs_dev")
-                # a log with a non-zero status has all-zero counters, so the sum counts exactly the logs with status 0
-                res = torch.cat([out.sum(0), status.to(torch.int64)]).cpu().numpy()
-                for name, v in zip(names, res[:len(names)]):
-                    total[name] += int(v)
-                st = res[len(names):]
+                sums, st = _stat_logs_dev(L, D, seats, dev, names)
+                for name, v in sums.items():
+                    total[name] += v
                 host += [T.files[j] for j in counted if st[j] != 0]
             for k in sorted(host):
                 host_total = host_total + _host_log_stat(chunk[k], player_name)
     return Stat(**total) + host_total
+
+
+def _stat_logs_dev(L, D, seats, dev, names):
+    """k_stat_logs over the decoded logs D (validate_logs.DecodedLogs with deltas) for the seat masks `seats` (uint8 [n]) ->
+    ({counter: sum over the logs with status 0}, status int32 [n]): the counters are summed on the device, and the sums and
+    statuses come back in one copy"""
+    import torch
+
+    from . import _lib
+
+    n = len(seats)
+    out = torch.empty((n, len(names)), dtype=torch.int64, device=dev)
+    status = torch.empty(n, dtype=torch.int32, device=dev)
+    d_seats = torch.from_numpy(seats).to(dev)
+    ptr = lambda t: t.data_ptr() if t.numel() else None
+    _lib.check(L.mjx_stat_logs_dev(n, ptr(D.hdr), D.offs[0].data_ptr(), D.offs[1].data_ptr(), D.hdr.numel(),
+                                   ptr(D.kyoku), D.offs[2].data_ptr(), D.kyoku.numel(), ptr(D.deltas), ptr(D.has_deltas),
+                                   d_seats.data_ptr(), out.data_ptr(), status.data_ptr(),
+                                   torch.cuda.current_stream(dev).cuda_stream), "mjx_stat_logs_dev")
+    # a log with a non-zero status has all-zero counters, so the sum counts exactly the logs with status 0
+    res = torch.cat([out.sum(0), status.to(torch.int64)]).cpu().numpy()
+    return {name: int(v) for name, v in zip(names, res[:len(names)])}, res[len(names):]
+
+
+def _game_events(games, g):
+    """the events of self-play game g's written log, decoded on the host (mjai_log.decode_events between the start_game the writer
+    writes and an end_game); RuntimeError naming the game and its seed, as selfplay.decode_games raises, for an overflowed log or
+    words decode_events rejects"""
+    import numpy as np
+
+    from .mjai_log import decode_events
+
+    n, seed = int(games.lens[g]), games.seeds[g]
+    if n < 0 or n > games.log_cap:
+        raise RuntimeError(f"self-play game {g} (seed {seed[0]}, {seed[1]}): event log overflow: {n} words > capacity {games.log_cap}")
+    try:
+        events = decode_events(games.words[g, :n].cpu().numpy().view(np.uint64))
+    except (ValueError, IndexError, KeyError) as e:
+        raise RuntimeError(f"self-play game {g} (seed {seed[0]}, {seed[1]}): corrupt event log: its words are not a sequence of "
+                           f"arena events ({type(e).__name__}: {e})") from e
+    return [games.first_event(g)] + events + [{"type": "end_game"}]
+
+
+def _host_games_stat(games, items) -> Stat:
+    """Stat.from_game over the host-decoded events of every (game, seat mask) in `items`"""
+    total = Stat()
+    for g, mask in items:
+        events = _game_events(games, g)
+        for s in range(4):
+            if mask >> s & 1:
+                total = total + Stat.from_game(events, s)
+    return total
 
 
 def main(argv=None) -> int:
