@@ -13,17 +13,25 @@ the reference's state file: `mortal` in mortal/model.py's key layout, `current_d
 ordered by the reference's sorted parameter names, so the optimizer state lines up index for index), `scheduler`, `scaler`,
 `steps`, `timestamp`, `best_perf`, `config`. State files move between the two trainers both ways.
 
-Online training replaces the reference's parameter server and self-play clients with one sequential loop in one process, the
-reference's `force_sequential = true`. Each round plays `player.TrainPlayer.train_play_games` sessions with the current parameters
-until at least `[online.server] capacity` games are held, logging each session's rankings and the `[online] history_window`
-moving average as mortal/client.py does. It then runs one `selfplay.SelfPlayDatasetsIter` over those games (the trainee's seats,
-the `[dataset]` flags), which yields what FileDatasetsIter yields over their written logs, so no log is written. The step uses the
-online loss, dqn + next_rank * next_rank_weight with no CQL term (mortal/train.py:236-238), and saves and test-plays as offline.
+Online training without `[online] actor_devices` replaces the reference's parameter server and self-play clients with one
+sequential loop in one process, the reference's `force_sequential = true`. Each round plays `player.TrainPlayer.train_play_games`
+sessions with the current parameters until at least `[online.server] capacity` games are held, logging each session's rankings
+and the `[online] history_window` moving average as mortal/client.py does. It then runs one `selfplay.SelfPlayDatasetsIter` over
+those games (the trainee's seats, the `[dataset]` flags), which yields what FileDatasetsIter yields over their written logs, so no
+log is written. The step uses the online loss, dqn + next_rank * next_rank_weight with no CQL term (mortal/train.py:236-238), and saves and test-plays as offline.
 Resuming from a state saved offline loads the weights, scaler, best_perf and steps, and starts a fresh optimizer and scheduler
-(mortal/train.py:106-118). These keys are read and have no effect: `submit_every` (no client plays during training),
-`force_sequential` (the loop is sequential), `[online.remote]`, `buffer_dir` and `drain_dir` (no files or sockets), and
-`[online] enable_compile`. The reference exits after a test play and respawns the trainer, a workaround for a hang in its
-process model; this loop simply continues.
+(mortal/train.py:106-118). In this loop these keys are read and have no effect: `submit_every` (no client plays during
+training) and `force_sequential` (the loop is sequential).
+
+With `[online] actor_devices = ["cuda:1", ...]` (one self-play actor process per entry, the trainer's own device allowed),
+`train_online` runs the reference's topology instead (mortal_b200.online): the actors play mortal/client.py's loop beside the
+trainer, which holds mortal/server.py's state, publishes its parameters where mortal/train.py submits them (idle at start, every
+`submit_every` steps, at a save off a submit, idle after each pass) and trains one pass per drain; `force_sequential` and
+`capacity` act as in the reference's server. Games and parameters stay on the GPUs (CUDA IPC).
+
+In both modes `[online.remote]`, `buffer_dir` and `drain_dir` (no files or sockets) and `[online] enable_compile` are read and
+have no effect. The reference exits after a test play and respawns the trainer, a workaround for a hang in its process model;
+these loops simply continue.
 
 Differences from the reference, stated rather than hidden:
 - `train()` raises ValueError for `online = true`: the online loop is `train_online`.
@@ -82,6 +90,15 @@ def check_online_config(config):
     capacity = config["online"]["server"]["capacity"]
     if capacity < 1:
         raise ValueError(f"[online.server] capacity must be at least 1, got {capacity}")
+    actor_devices = config["online"].get("actor_devices")
+    if actor_devices:
+        from .online import parse_actor_devices
+
+        n, per_session = len(parse_actor_devices(actor_devices)), play["games"] // 4 * 4
+        if config["online"]["server"].get("force_sequential", False) and n * per_session < capacity:
+            raise ValueError(f"force_sequential = true with {n} actor(s) x {per_session} games per session = {n * per_session} "
+                             f"games per round, fewer than [online.server] capacity = {capacity}: every actor would wait for "
+                             "an idle publish while the trainer waits for capacity games")
 
 
 def _check_common(config):
@@ -161,6 +178,8 @@ class _Trainer:
         self.version = version = control["version"]
         self.batch_size, self.opt_step_every = control["batch_size"], control["opt_step_every"]
         self.save_every, self.test_every = control["save_every"], control["test_every"]
+        self.submit_every = control.get("submit_every")
+        self.publish = None  # with self-play actors: publish(is_idle) hands the parameters over (mortal_b200.online)
         self.test_games = config["test_play"]["games"]
         self.min_q_weight = config["cql"]["min_q_weight"]
         self.next_rank_weight = config["aux"]["next_rank_weight"]
@@ -257,6 +276,8 @@ class _Trainer:
             self.scaler.update()
             self.optimizer.zero_grad(set_to_none=True)
         self.scheduler.step()
+        if self.publish is not None and self.total % self.submit_every == 0:  # mortal/train.py:271-273
+            self.publish(False)
         if self.total % self.save_every == 0:
             self._save()
 
@@ -285,6 +306,8 @@ class _Trainer:
             "config": self.config,
         }
         torch.save(state, self.state_file)
+        if self.publish is not None and total % self.submit_every != 0:  # mortal/train.py:312-314
+            self.publish(False)
 
         if total % test_every == 0:
             best_perf = self.best_perf
@@ -353,21 +376,46 @@ def train(config, steps=None):
     return T.mortal, T.dqn, T.aux_net, T.optimizer, T.total
 
 
-def train_online(config, rounds=None, steps=None):
-    """mortal/train.py with `online = true`, as one sequential loop in this process (module docstring). `rounds` bounds the call
-    to that many rounds of self-play + training, `steps` to that many training steps (None: no bound; the loop then runs until
-    interrupted). Returns (brain, dqn, aux_net, optimizer, total steps)."""
+def _train_pass(T, config, grp, games, steps, done):
+    """one SelfPlayDatasetsIter pass over `games` (the trainee's seats, the [dataset] flags), stopping once `done` reaches `steps`
+    -> the new `done`"""
+    from .selfplay import SelfPlayDatasetsIter
+
+    ds = config["dataset"]
+    data = SelfPlayDatasetsIter(T.version, games, config["env"]["pts"], file_batch_size=ds["file_batch_size"],
+                                reserve_ratio=ds["reserve_ratio"], player_names=["trainee"], num_epochs=ds["num_epochs"],
+                                enable_augmentation=ds["enable_augmentation"], augmented_first=ds["augmented_first"], grp=grp,
+                                batch_size=T.batch_size, device=T.device.index)
+    for batch in data:
+        if steps is not None and done >= steps:
+            break
+        if batch[0].shape[0] != T.batch_size:
+            continue  # a final short batch is not trained on (mortal/train.py:389-422)
+        T.step(*batch)
+        done += 1
+    return done
+
+
+def train_online(config, rounds=None, steps=None, monitor=None):
+    """mortal/train.py with `online = true` (module docstring). Without `[online] actor_devices`, one sequential loop in this
+    process: `rounds` bounds the call to that many rounds of self-play + training. With it, self-play actors beside the trainer
+    (mortal_b200.online.train_concurrent): `rounds` counts the drains trained on, and `monitor(kind, **info)` receives the
+    parameter server's publish, submit and drain events (mortal_b200.online.Server). `steps` bounds either to that many training
+    steps (None: no bound; the loop then runs until interrupted). Returns (brain, dqn, aux_net, optimizer, total steps)."""
     from .player import TrainPlayer
-    from .selfplay import SelfPlayDatasetsIter, SelfPlayGames
+    from .selfplay import SelfPlayGames
 
     check_online_config(config)
+    if config["online"].get("actor_devices"):
+        from .online import train_concurrent
+
+        return train_concurrent(config, rounds=rounds, steps=steps, monitor=monitor)
     online_cfg = config["online"]
     server = online_cfg["server"]
     capacity, history_window = server["capacity"], online_cfg["history_window"]
     _ = (config["control"].get("submit_every"), server.get("force_sequential"), server.get("buffer_dir"),  # read, no effect
          server.get("drain_dir"), online_cfg.get("remote"), online_cfg.get("enable_compile"))       # (module docstring)
     T = _Trainer(config, online=True)
-    ds = config["dataset"]
     grp = _load_grp(config)
     train_player = TrainPlayer(config)
     pts = np.array([90, 45, 0, -135])  # mortal/client.py:31, for the log lines only
@@ -391,18 +439,8 @@ def train_online(config, rounds=None, steps=None):
         del held
         logging.info(f"round {rounds_done + 1}: {len(games):,} games; total steps: {T.total:,} "
                      f"(~{(T.test_every - T.total % T.test_every) % T.test_every:,})")
-        data = SelfPlayDatasetsIter(T.version, games, config["env"]["pts"], file_batch_size=ds["file_batch_size"],
-                                    reserve_ratio=ds["reserve_ratio"], player_names=["trainee"], num_epochs=ds["num_epochs"],
-                                    enable_augmentation=ds["enable_augmentation"], augmented_first=ds["augmented_first"], grp=grp,
-                                    batch_size=T.batch_size, device=T.device.index)
-        for batch in data:
-            if steps is not None and done >= steps:
-                break
-            if batch[0].shape[0] != T.batch_size:
-                continue  # a final short batch is not trained on (mortal/train.py:389-422)
-            T.step(*batch)
-            done += 1
-        del data, games  # the round's games are freed before the next round plays
+        done = _train_pass(T, config, grp, games, steps, done)
+        del games  # the round's games are freed before the next round plays
         rounds_done += 1
     T.check_actions()
     return T.mortal, T.dqn, T.aux_net, T.optimizer, T.total
