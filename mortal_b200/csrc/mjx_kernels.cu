@@ -9,6 +9,7 @@
 
 #include "../../include/mjx.h"
 #include "../../include/mjx_review.h"
+#include "../../include/mjx_train_ranks.h"
 #include "mjx_sp.cuh"
 #include "mjx_policy.cuh"
 #include "mjx_replay.cuh"
@@ -2600,6 +2601,71 @@ int mjx_train_bn_mish_bwd(int dtype, const void* x, const void* dout, const floa
         mjx_train::k_bn_mish_bwd_dx<T><<<train_grid(n), 256, 0, s>>>((const T*)x, (const T*)dout, save_mean, save_invstd, gamma,
                                                                      beta, coef, (T*)dx, n, C);
     });
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+int mjx_train_bn_local_stats(int dtype, const void* x, int rows, int channels, int rank, int world, double* stats, float* scratch,
+                             void* stream) {
+    if (!train_shape_ok(dtype, rows, channels) || !x || !stats || !scratch || world < 1 || rank < 0 || rank >= world ||
+        (uintptr_t)stats % 8)
+        return fail(MJX_ERR_ARG, "mjx_train_bn_local_stats: bad arguments (0 <= rank < world, stats 8-byte aligned)");
+    cudaStream_t s = (cudaStream_t)stream;
+    const int G = mjx_train::bn_blocks(rows), R = mjx_train::bn_rows_per_block(rows), C = channels;
+    const int threads = mjx_train::bn_lanes(C) * C;
+    MJX_TRAIN_DISPATCH(dtype, mjx_train::k_bn_stats<T><<<G, threads, 0, s>>>((const T*)x, rows, C, R, scratch));
+    mjx_train::k_bn_local_stats<<<C, mjx_train::FIN_THREADS, 0, s>>>(scratch, G, C, rank, stats);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+int mjx_train_bn_mish_fwd_ranks(int dtype, const void* x, const float* gamma, const float* beta, float* running_mean,
+                                float* running_var, float* save_mean, float* save_invstd, void* out, int rows, int channels, float eps,
+                                float momentum, const double* stats, int world, void* stream) {
+    if (!train_shape_ok(dtype, rows, channels) || !x || !gamma || !beta || !running_mean || !running_var || !save_mean ||
+        !save_invstd || !out || !stats || world < 1 || (uintptr_t)stats % 8)
+        return fail(MJX_ERR_ARG, "mjx_train_bn_mish_fwd_ranks: bad arguments (world >= 1, stats 8-byte aligned)");
+    cudaStream_t s = (cudaStream_t)stream;
+    const int C = channels, FT = mjx_train::FIN_THREADS;
+    mjx_train::k_bn_finalize_ranks<<<(C + FT - 1) / FT, FT, 0, s>>>(stats, world, C, eps, momentum, running_mean, running_var,
+                                                                   save_mean, save_invstd);
+    const int n = rows * C;
+    MJX_TRAIN_DISPATCH(dtype, mjx_train::k_bn_mish_apply<T><<<train_grid(n), 256, 0, s>>>((const T*)x, save_mean, save_invstd, gamma,
+                                                                                          beta, (T*)out, n, C));
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+int mjx_train_bn_bwd_local_sums(int dtype, const void* x, const void* dout, const float* gamma, const float* beta,
+                                const float* save_mean, const float* save_invstd, int rows, int channels, int rank, int world,
+                                double* sums, float* scratch, void* stream) {
+    if (!train_shape_ok(dtype, rows, channels) || !x || !dout || !gamma || !beta || !save_mean || !save_invstd || !sums || !scratch ||
+        world < 1 || rank < 0 || rank >= world || (uintptr_t)sums % 8 || (uintptr_t)scratch % 8)
+        return fail(MJX_ERR_ARG, "mjx_train_bn_bwd_local_sums: bad arguments (0 <= rank < world, sums and scratch 8-byte aligned)");
+    cudaStream_t s = (cudaStream_t)stream;
+    const int G = mjx_train::bn_blocks(rows), R = mjx_train::bn_rows_per_block(rows), C = channels;
+    const int threads = mjx_train::bn_lanes(C) * C;
+    double* part = (double*)scratch;
+    MJX_TRAIN_DISPATCH(dtype, mjx_train::k_bn_mish_bwd_sums<T><<<G, threads, 0, s>>>((const T*)x, (const T*)dout, save_mean,
+                                                                                     save_invstd, gamma, beta, rows, C, R, part));
+    mjx_train::k_bn_bwd_local_sums<<<C, mjx_train::FIN_THREADS, 0, s>>>(part, G, C, rank, sums);
+    CU(cudaGetLastError());
+    return MJX_OK;
+}
+int mjx_train_bn_mish_bwd_ranks(int dtype, const void* x, const void* dout, const float* gamma, const float* beta,
+                                const float* save_mean, const float* save_invstd, void* dx, float* dgamma, float* dbeta, int rows,
+                                int channels, const double* sums, int rank, int world, long long total_rows, float* scratch,
+                                void* stream) {
+    if (!train_shape_ok(dtype, rows, channels) || !x || !dout || !gamma || !beta || !save_mean || !save_invstd || !dx || !dgamma ||
+        !dbeta || !sums || !scratch || world < 1 || rank < 0 || rank >= world || total_rows < rows || (uintptr_t)sums % 8)
+        return fail(MJX_ERR_ARG, "mjx_train_bn_mish_bwd_ranks: bad arguments (0 <= rank < world, total_rows >= rows, sums 8-byte "
+                                 "aligned)");
+    cudaStream_t s = (cudaStream_t)stream;
+    const int C = channels, FT = mjx_train::FIN_THREADS;
+    float* coef = scratch;  // 3 * C floats
+    mjx_train::k_bn_bwd_finalize_ranks<<<(C + FT - 1) / FT, FT, 0, s>>>(sums, world, rank, C, (double)total_rows, gamma, save_invstd,
+                                                                       dgamma, dbeta, coef);
+    const int n = rows * C;
+    MJX_TRAIN_DISPATCH(dtype, mjx_train::k_bn_mish_bwd_dx<T><<<train_grid(n), 256, 0, s>>>((const T*)x, (const T*)dout, save_mean,
+                                                                                           save_invstd, gamma, beta, coef, (T*)dx, n,
+                                                                                           C));
     CU(cudaGetLastError());
     return MJX_OK;
 }

@@ -1,7 +1,8 @@
 // mortal_b200 — fused kernels for training the policy net (mortal/train.py:228-248 over mortal/model.py's Brain / DQN / AuxNet,
 // restated in mortal_b200/model.py and mortal_b200/train_ops.py). The convolutions and Linear layers stay with cuDNN / cuBLAS;
 // what autograd runs around them as many small elementwise and reduction kernels is done here:
-//   - training-mode BatchNorm + Mish, forward and backward (every pre-activation of a block and the trunk's last BN + Mish);
+//   - training-mode BatchNorm + Mish, forward and backward (every pre-activation of a block and the trunk's last BN + Mish), also
+//     split around an exchange of per-channel partials so that data-parallel ranks normalise with the global batch's statistics;
 //   - the channel gate's pooling and `y * g + x`, and their backward;
 //   - the dueling combine, the DQN / CQL / next-rank losses and their gradients.
 // Activations are channels-last [rows = batch * length, channels], stored as float or __half, with fp32 arithmetic. Every
@@ -86,7 +87,40 @@ __device__ __forceinline__ void chan_merge(double& n, double& mean, double& m2, 
     m2 += m2b + d * d * (n * nb / nt);
     n = nt;
 }
-// one block per channel: thread t merges partials t, t + FIN_THREADS, ... in order, then a pairwise tree in fixed order
+// channel c of one block: thread t merges partials t, t + FIN_THREADS, ... in order, then a pairwise tree in fixed order; the
+// result is in thread 0's n / mean / m2
+__device__ __forceinline__ void bn_merge_parts(const float* __restrict__ part, int G, int C, int c, double* sn, double* sm,
+                                               double* s2, double& n, double& mean, double& m2) {
+    const int t = threadIdx.x;
+    n = 0.; mean = 0.; m2 = 0.;
+    for (int g = t; g < G; g += FIN_THREADS) {
+        const float* p = part + (size_t)g * 4 * C;
+        chan_merge(n, mean, m2, p[c], (double)p[C + c] + (double)p[2 * C + c], p[3 * C + c]);
+    }
+    sn[t] = n; sm[t] = mean; s2[t] = m2;
+    __syncthreads();
+    for (int h = FIN_THREADS / 2; h; h >>= 1) {
+        if (t < h) {
+            chan_merge(n, mean, m2, sn[t + h], sm[t + h], s2[t + h]);
+            sn[t] = n; sm[t] = mean; s2[t] = m2;
+        }
+        __syncthreads();
+    }
+}
+// the batch statistics of channel c from its merged (n, mean, M2), and the running statistics' update
+__device__ __forceinline__ void bn_write_stats(int c, int C, double n, double mean, double m2, float eps, float momentum,
+                                               float* __restrict__ running_mean, float* __restrict__ running_var,
+                                               float* __restrict__ save_mean, float* __restrict__ save_invstd) {
+    const float var = (float)(m2 / n);
+    const float hi = (float)mean;
+    save_mean[c] = hi;
+    save_mean[C + c] = (float)(mean - (double)hi);
+    save_invstd[c] = 1.f / sqrtf(var + eps);
+    const float unbiased = (float)(m2 / (n - 1.));
+    running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * (float)mean;
+    running_var[c] = (1.f - momentum) * running_var[c] + momentum * unbiased;
+}
+// one block per channel
 __global__ void __launch_bounds__(FIN_THREADS) k_bn_finalize(const float* __restrict__ part, int G, int C, int n_rows, float eps,
                                                              float momentum, int training, float* __restrict__ running_mean,
                                                              float* __restrict__ running_var, float* __restrict__ save_mean,
@@ -101,29 +135,44 @@ __global__ void __launch_bounds__(FIN_THREADS) k_bn_finalize(const float* __rest
         }
         return;
     }
-    double n = 0., mean = 0., m2 = 0.;
-    for (int g = t; g < G; g += FIN_THREADS) {
-        const float* p = part + (size_t)g * 4 * C;
-        chan_merge(n, mean, m2, p[c], (double)p[C + c] + (double)p[2 * C + c], p[3 * C + c]);
-    }
-    sn[t] = n; sm[t] = mean; s2[t] = m2;
-    __syncthreads();
-    for (int h = FIN_THREADS / 2; h; h >>= 1) {
-        if (t < h) {
-            chan_merge(n, mean, m2, sn[t + h], sm[t + h], s2[t + h]);
-            sn[t] = n; sm[t] = mean; s2[t] = m2;
-        }
-        __syncthreads();
-    }
+    double n, mean, m2;
+    bn_merge_parts(part, G, C, c, sn, sm, s2, n, mean, m2);
     if (t) return;
-    const float var = (float)(m2 / n);
-    const float hi = (float)mean;
-    save_mean[c] = hi;
-    save_mean[C + c] = (float)(mean - (double)hi);
-    save_invstd[c] = 1.f / sqrtf(var + eps);
-    const float unbiased = (float)(m2 / (n - 1.));
-    running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * (float)mean;
-    running_var[c] = (1.f - momentum) * running_var[c] + momentum * unbiased;
+    bn_write_stats(c, C, n, mean, m2, eps, momentum, running_mean, running_var, save_mean, save_invstd);
+}
+
+// ---- BatchNorm statistics across ranks (data-parallel training) ----------------------------------------------------------------
+// The forward and backward are split where the ranks exchange per-channel partials: each rank merges its own rows in the order
+// k_bn_finalize / k_bn_bwd_finalize use and writes row `rank` of a [world][.][C] double buffer (the others zero); a sum over
+// ranks of those buffers (all_reduce SUM: adding exact zeros is exact) gives every rank every row; each rank then merges the
+// rows in rank order, so all ranks compute bit-identical statistics. Row 0 starts the merge (not n = 0, a sum of 0.0), so with
+// world = 1 the result is the single-process one bit for bit.
+
+// stats[rank][3][C] = (n, mean, M2) of this rank's rows (k_bn_finalize's merge, before its float write); one block per channel
+__global__ void __launch_bounds__(FIN_THREADS) k_bn_local_stats(const float* __restrict__ part, int G, int C, int rank,
+                                                                double* __restrict__ stats) {
+    __shared__ double sn[FIN_THREADS], sm[FIN_THREADS], s2[FIN_THREADS];
+    const int c = blockIdx.x;
+    double n, mean, m2;
+    bn_merge_parts(part, G, C, c, sn, sm, s2, n, mean, m2);
+    if (threadIdx.x) return;
+    double* o = stats + (size_t)rank * 3 * C;
+    o[c] = n; o[C + c] = mean; o[2 * C + c] = m2;
+}
+
+// merge the world rows of stats [world][3][C] in rank order and write the statistics as k_bn_finalize does; one thread per channel
+__global__ void __launch_bounds__(FIN_THREADS) k_bn_finalize_ranks(const double* __restrict__ stats, int world, int C, float eps,
+                                                                   float momentum, float* __restrict__ running_mean,
+                                                                   float* __restrict__ running_var, float* __restrict__ save_mean,
+                                                                   float* __restrict__ save_invstd) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    double n = stats[c], mean = stats[C + c], m2 = stats[2 * C + c];
+    for (int r = 1; r < world; r++) {
+        const double* p = stats + (size_t)r * 3 * C;
+        chan_merge(n, mean, m2, p[c], p[C + c], p[2 * C + c]);
+    }
+    bn_write_stats(c, C, n, mean, m2, eps, momentum, running_mean, running_var, save_mean, save_invstd);
 }
 
 // out = mish(gamma * (x - mean) * invstd + beta), mean = mean[c] + mean[C + c]
@@ -168,12 +217,9 @@ __global__ void __launch_bounds__(256) k_bn_mish_bwd_sums(const T* __restrict__ 
 
 // dbeta = sum dz, dgamma = sum dz * xhat (double, one block per channel, an order fixed by G), and the coefficients of
 // dx = k1 dz - k2 - xhat k3: k1 = gamma invstd; k2 = k1 sum dz / N, k3 = k1 sum(dz xhat) / N in training, 0 for a frozen BN
-__global__ void __launch_bounds__(FIN_THREADS) k_bn_bwd_finalize(const double* __restrict__ part, int G, int C, int n_rows, int training,
-                                                                 const float* __restrict__ gamma, const float* __restrict__ invstd,
-                                                                 float* __restrict__ dgamma, float* __restrict__ dbeta,
-                                                                 float* __restrict__ coef) {
-    __shared__ double s1[FIN_THREADS], s2[FIN_THREADS];
-    const int c = blockIdx.x, t = threadIdx.x;
+// channel c of one block: the block partials summed in an order fixed by G, the result in s1[0] / s2[0]
+__device__ __forceinline__ void bn_sum_parts(const double* __restrict__ part, int G, int C, int c, double* s1, double* s2) {
+    const int t = threadIdx.x;
     double a1 = 0., a2 = 0.;
     for (int g = t; g < G; g += FIN_THREADS) {
         a1 += part[(size_t)g * 2 * C + c];
@@ -185,14 +231,58 @@ __global__ void __launch_bounds__(FIN_THREADS) k_bn_bwd_finalize(const double* _
         if (t < h) { s1[t] += s1[t + h]; s2[t] += s2[t + h]; }
         __syncthreads();
     }
-    if (t) return;
-    a1 = s1[0]; a2 = s2[0];
-    dbeta[c] = (float)a1;
-    dgamma[c] = (float)a2;
+}
+// the dx coefficients of channel c from sum dz (a1) and sum dz xhat (a2) over n_rows rows
+__device__ __forceinline__ void bn_write_coef(int c, int C, double a1, double a2, double n_rows, int training,
+                                              const float* __restrict__ gamma, const float* __restrict__ invstd,
+                                              float* __restrict__ coef) {
     const float k1 = gamma[c] * invstd[c];
     coef[c] = k1;
     coef[C + c] = training ? (float)((double)k1 * a1 / n_rows) : 0.f;
     coef[2 * C + c] = training ? (float)((double)k1 * a2 / n_rows) : 0.f;
+}
+__global__ void __launch_bounds__(FIN_THREADS) k_bn_bwd_finalize(const double* __restrict__ part, int G, int C, int n_rows, int training,
+                                                                 const float* __restrict__ gamma, const float* __restrict__ invstd,
+                                                                 float* __restrict__ dgamma, float* __restrict__ dbeta,
+                                                                 float* __restrict__ coef) {
+    __shared__ double s1[FIN_THREADS], s2[FIN_THREADS];
+    const int c = blockIdx.x;
+    bn_sum_parts(part, G, C, c, s1, s2);
+    if (threadIdx.x) return;
+    const double a1 = s1[0], a2 = s2[0];
+    dbeta[c] = (float)a1;
+    dgamma[c] = (float)a2;
+    bn_write_coef(c, C, a1, a2, n_rows, training, gamma, invstd, coef);
+}
+
+// sums[rank][2][C] = (sum dz, sum dz xhat) of this rank's rows, k_bn_bwd_finalize's order; one block per channel
+__global__ void __launch_bounds__(FIN_THREADS) k_bn_bwd_local_sums(const double* __restrict__ part, int G, int C, int rank,
+                                                                   double* __restrict__ sums) {
+    __shared__ double s1[FIN_THREADS], s2[FIN_THREADS];
+    const int c = blockIdx.x;
+    bn_sum_parts(part, G, C, c, s1, s2);
+    if (threadIdx.x) return;
+    double* o = sums + (size_t)rank * 2 * C;
+    o[c] = s1[0]; o[C + c] = s2[0];
+}
+
+// the training-mode coefficients from the rows of sums [world][2][C] added in rank order over all ranks' total_rows rows, and
+// dgamma / dbeta from this rank's own row (a data-parallel gradient all-reduce sums or averages them); one thread per channel
+__global__ void __launch_bounds__(FIN_THREADS) k_bn_bwd_finalize_ranks(const double* __restrict__ sums, int world, int rank, int C,
+                                                                       double total_rows, const float* __restrict__ gamma,
+                                                                       const float* __restrict__ invstd, float* __restrict__ dgamma,
+                                                                       float* __restrict__ dbeta, float* __restrict__ coef) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    double a1 = sums[c], a2 = sums[C + c];
+    for (int r = 1; r < world; r++) {
+        a1 += sums[(size_t)r * 2 * C + c];
+        a2 += sums[(size_t)r * 2 * C + C + c];
+    }
+    const double* own = sums + (size_t)rank * 2 * C;
+    dbeta[c] = (float)own[c];
+    dgamma[c] = (float)own[C + c];
+    bn_write_coef(c, C, a1, a2, total_rows, 1, gamma, invstd, coef);
 }
 
 template <class T>

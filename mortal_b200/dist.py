@@ -14,6 +14,13 @@ def shard_seeds(seed_start, seed_count_per_rank: int, rank: int, games_per_seed:
     return nonces, keys
 
 
+def seed_block(seed_count: int, rank: int, world: int):
+    """(first seed offset, seed count) of the rank's contiguous block of `seed_count` seeds split over `world` ranks: the first
+    seed_count % world ranks take one seed more, so the blocks cover every seed once, in rank order"""
+    base, extra = divmod(seed_count, world)
+    return rank * base + min(rank, extra), base + (rank < extra)
+
+
 def gather_returns(scores, ranks, device=None):
     """all_gather of {scores i32[n,4], ranks u8[n,4]} -> (scores [world*n,4], ranks [world*n,4]) on every rank.
     Works with any initialised torch.distributed backend (nccl on GPUs, gloo in the CPU tests)."""

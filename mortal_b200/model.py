@@ -157,11 +157,13 @@ class Brain(nn.Module):
         self._freeze_bn = bool(value)
         return self.train(self.training)
 
-    def forward_train(self, obs):
+    def forward_train(self, obs, group=None):
         """phi [B, 1024] of versions 2-4 as `forward` computes it, for training: the convolutions are cuDNN on channels-last (1 x 3)
         views of the Conv1d weights, every BatchNorm + Mish of the trunk and every channel gate + residual run as the fused
         kernels of mortal_b200.train_ops (float32, or float16 under torch.autocast). Gradients reach this module's own parameters;
-        the BatchNorms update their running statistics when in train mode (not frozen), as `forward` does."""
+        the BatchNorms update their running statistics when in train mode (not frozen), as `forward` does. With a
+        torch.distributed `group` of several data-parallel ranks (each passing a batch of the same shape), training-mode
+        BatchNorm normalises with the statistics of all the ranks' batches together (train_ops.bn_mish)."""
         from . import train_ops
 
         if self.version == 1:
@@ -173,10 +175,10 @@ class Brain(nn.Module):
         w = lambda conv: conv.weight.unsqueeze(2)  # [Cout, Cin, 1, 3] view: autograd gives the Conv1d weight's gradient
         x = F.conv2d(obs.unsqueeze(2).contiguous(memory_format=torch.channels_last), w(self.stem), padding=(0, 1))
         for blk in self.blocks:
-            y = F.conv2d(train_ops.bn_mish(x, blk.bn1), w(blk.conv1), padding=(0, 1))
-            y = F.conv2d(train_ops.bn_mish(y, blk.bn2), w(blk.conv2), padding=(0, 1))
+            y = F.conv2d(train_ops.bn_mish(x, blk.bn1, group=group), w(blk.conv1), padding=(0, 1))
+            y = F.conv2d(train_ops.bn_mish(y, blk.bn2, group=group), w(blk.conv2), padding=(0, 1))
             x = train_ops.gate_residual(y, x, blk.gate)
-        x = F.mish(F.conv2d(train_ops.bn_mish(x, self.bn), w(self.neck), self.neck.bias, padding=(0, 1)))
+        x = F.mish(F.conv2d(train_ops.bn_mish(x, self.bn, group=group), w(self.neck), self.neck.bias, padding=(0, 1)))
         return F.mish(self.fc(x.flatten(1)))
 
     def forward(self, obs, invisible_obs=None):

@@ -24,10 +24,11 @@ from os import path
 import numpy as np
 import torch
 
+from .dist import seed_block
 from .engine import DeviceEngine
 from .libriichi.arena import OneVsThree
 from .model import load_mortal
-from .stat import Stat
+from .stat import COUNTERS, Stat
 
 
 class TestPlayer:
@@ -42,16 +43,41 @@ class TestPlayer:
         self.log_dir = path.abspath(config["test_play"]["log_dir"])
         self.cudnn_benchmark = config["control"].get("enable_cudnn_benchmark", False)
 
-    def test_play(self, seed_count, mortal, dqn, device):
+    def test_play(self, seed_count, mortal, dqn, device, group=None):
         """`seed_count` seeds x 4 games from seed (10000, 0x2000), the challenger in each seat once; logs in `log_dir` (emptied
-        first); returns the challenger's Stat"""
+        first); returns the challenger's Stat.
+
+        With a torch.distributed `group` of several data-parallel ranks (all sharing `log_dir`'s file system), each rank plays its
+        contiguous block of the seeds (dist.seed_block) on `device` and writes its games' logs under the names one process would
+        give them; the Stat is the sum over the ranks of each rank's Stat of its own recorded games, the same on every rank."""
+        import torch.distributed as dist
+
+        world = dist.get_world_size(group) if group is not None else 1
         torch.backends.cudnn.benchmark = False
         engine_chal = DeviceEngine(mortal, dqn, version=self.chal_version, device=device, enable_amp=True, name="mortal")
-        if path.isdir(self.log_dir):
-            shutil.rmtree(self.log_dir)
-        env = OneVsThree(disable_progress_bar=True, log_dir=self.log_dir, device=device.index or 0)
-        env.py_vs_py(challenger=engine_chal, champion=self.baseline_engine, seed_start=(10000, 0x2000), seed_count=seed_count)
-        stat = Stat.from_dir(self.log_dir, "mortal", disable_progress_bar=True)
+        if world == 1:
+            if path.isdir(self.log_dir):
+                shutil.rmtree(self.log_dir)
+            env = OneVsThree(disable_progress_bar=True, log_dir=self.log_dir, device=device.index or 0)
+            env.py_vs_py(challenger=engine_chal, champion=self.baseline_engine, seed_start=(10000, 0x2000), seed_count=seed_count)
+            stat = Stat.from_dir(self.log_dir, "mortal", disable_progress_bar=True)
+        else:
+            rank = dist.get_rank(group)
+            if rank == 0 and path.isdir(self.log_dir):
+                shutil.rmtree(self.log_dir)
+            dist.barrier(group=group)
+            start, count = seed_block(seed_count, rank, world)
+            stat = Stat()
+            if count:
+                env = OneVsThree(disable_progress_bar=True, log_dir=self.log_dir, device=device.index or 0)
+                env.record_games = True
+                env.py_vs_py(challenger=engine_chal, champion=self.baseline_engine, seed_start=(10000 + start, 0x2000),
+                             seed_count=count)
+                stat = Stat.from_games(env.last_games, "mortal")
+                env.last_games = None
+            counters = torch.tensor([getattr(stat, c) for c in COUNTERS], dtype=torch.int64, device=device)
+            dist.all_reduce(counters, group=group)
+            stat = Stat(**dict(zip(COUNTERS, counters.tolist())))
         torch.backends.cudnn.benchmark = self.cudnn_benchmark
         return stat
 

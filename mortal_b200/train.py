@@ -33,6 +33,26 @@ In both modes `[online.remote]`, `buffer_dir` and `drain_dir` (no files or socke
 have no effect. The reference exits after a test play and respawns the trainer, a workaround for a hang in its process model;
 these loops simply continue.
 
+Data-parallel training: `torchrun --nproc-per-node=N -m mortal_b200.train [CONFIG]` starts one rank per GPU (NCCL, each rank on
+cuda:LOCAL_RANK for the trainer and `[baseline.test]`), and `train()` itself trains data-parallel whenever torch.distributed is
+initialised with more than one rank (NCCL or gloo). `[control] batch_size` stays the global batch: each of the W ranks trains on
+batch_size / W samples, and one step is still one optimizer update over batch_size samples.
+- Every training-mode BatchNorm normalises with the global batch's statistics (train_ops.bn_mish with the default group), so W
+  ranks train the model one GPU would at the same batch, up to rounding. Gradients are all-reduced and averaged once per optimizer
+  step, before unscale_ / clip_grad_norm_ / GradScaler.step; rank 0's initial or loaded weights are broadcast at the start, and
+  from then on parameters, BatchNorm statistics, optimizer and scaler state stay bitwise equal across the ranks.
+- Rank 0 builds or loads the file index, shuffles the list and broadcasts the permutation; rank r trains on the r-th contiguous
+  shard of ceil(len / W) files (the reference's worker_init_fn split) with its own FileDatasetsIter. An empty shard raises
+  ValueError on every rank. The ranks agree before each step (a host-side gloo collective) that every one holds a full batch;
+  training ends for all when one runs out.
+- The illegal-action check is all-reduced, so every rank raises the same ValueError. The loss line averages over the ranks. Only
+  rank 0 logs at INFO, writes `state_file` and copies `best_state_file`; the state file is the single-process one.
+- The test play splits its seeds into contiguous blocks, one per rank, each played on the rank's GPU into the same `log_dir`
+  (emptied by rank 0) under the file names a single-process run uses; the ranks' Stat counters are summed, so every rank takes
+  the same best_perf decision.
+- Refused with ValueError: a batch_size W does not divide, a `[baseline.test]` device other than the trainer's, and
+  `train_online` (online training is not data-parallel).
+
 Differences from the reference, stated rather than hidden:
 - `train()` raises ValueError for `online = true`: the online loop is `train_online`.
 - Version 1 raises ValueError: its Brain returns (mu, logsig), which the reference's train.py cannot train either.
@@ -71,15 +91,26 @@ from .train_grp import load_config
 BEST_PERF = {"avg_rank": 4.0, "avg_pt": -135.0}
 
 
-def check_config(config):
-    """ValueError for what the offline trainer does not run (module docstring), before anything touches the device"""
+def check_config(config, world: int = 1):
+    """ValueError for what the offline trainer does not run (module docstring) with `world` data-parallel ranks, before anything
+    touches the device"""
     if config["control"].get("online", False):
         raise ValueError("online = true: online training runs in train_online(config), not train()")
     _check_common(config)
+    if world > 1:
+        batch_size = config["control"]["batch_size"]
+        if batch_size % world:
+            raise ValueError(f"[control] batch_size = {batch_size} is the global batch; {world} ranks must divide it")
+        trainer, test = torch.device(config["control"]["device"]), torch.device(config["baseline"]["test"]["device"])
+        if trainer != test:
+            raise ValueError(f"data-parallel training plays each rank's test games on its trainer's device, so [baseline.test] "
+                             f"device must be [control] device; got {test} and {trainer}")
 
 
-def check_online_config(config):
-    """ValueError for an online config train_online cannot run, before anything touches the device"""
+def check_online_config(config, world: int = 1):
+    """ValueError for an online config train_online cannot run (with `world` ranks), before anything touches the device"""
+    if world > 1:
+        raise ValueError(f"online training is not data-parallel: train_online runs in one process, got {world} ranks")
     _check_common(config)
     profile = os.environ.get("TRAIN_PLAY_PROFILE", "default")
     play = config.get("train_play", {}).get(profile)
@@ -160,6 +191,28 @@ def _file_list(ds, player_names_set):
     return file_list
 
 
+def world_info():
+    """(group, rank, world) of the initialised default torch.distributed group with more than one rank, else (None, 0, 1)"""
+    import torch.distributed as dist
+
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+        return dist.group.WORLD, dist.get_rank(), dist.get_world_size()
+    return None, 0, 1
+
+
+def shard(file_list, rank: int, world: int):
+    """the rank's contiguous block of ceil(len / world) files (the reference's worker_init_fn, mortal/dataloader.py:133-139)"""
+    per = -(-len(file_list) // world)
+    return file_list[rank * per:(rank + 1) * per]
+
+
+def check_shards(n_files: int, world: int):
+    """ValueError when a rank's shard of n_files files would be empty (every rank computes the same answer)"""
+    empty = [r for r in range(world) if not shard(range(n_files), r, world)]
+    if empty:
+        raise ValueError(f"{n_files} files cannot give each of {world} ranks a shard: rank(s) {empty} would have none")
+
+
 def _player_names(ds):
     names = set()
     for filename in ds.get("player_names_files", []):
@@ -175,8 +228,16 @@ class _Trainer:
     def __init__(self, config, online: bool):
         control = config["control"]
         self.config, self.online = config, online
+        self.group, self.rank, self.world = world_info()
+        self.flag_group = None  # a gloo group for host-side flags beside an NCCL default group
+        if self.world > 1:
+            import torch.distributed as dist
+
+            self.flag_group = self.group if dist.get_backend() == "gloo" else dist.new_group(backend="gloo")
+        self.info = logging.info if self.rank == 0 else logging.debug
         self.version = version = control["version"]
-        self.batch_size, self.opt_step_every = control["batch_size"], control["opt_step_every"]
+        # the rank's share of the global batch (check_config: the ranks divide it)
+        self.batch_size, self.opt_step_every = control["batch_size"] // self.world, control["opt_step_every"]
         self.save_every, self.test_every = control["save_every"], control["test_every"]
         self.submit_every = control.get("submit_every")
         self.publish = None  # with self-play actors: publish(is_idle) hands the parameters over (mortal_b200.online)
@@ -198,9 +259,9 @@ class _Trainer:
         self.mortal = mortal = Brain(version=version, **config["resnet"]).to(device)
         self.dqn = dqn = DQN(version=version).to(device)
         self.aux_net = aux_net = AuxNet((4,)).to(device)
-        logging.info(f"version: {version}")
+        self.info(f"version: {version}")
         for name, m in (("mortal", mortal), ("dqn", dqn), ("aux", aux_net)):
-            logging.info(f"{name} params: {sum(p.numel() for p in m.parameters() if p.requires_grad):,}")
+            self.info(f"{name} params: {sum(p.numel() for p in m.parameters() if p.requires_grad):,}")
         mortal.freeze_bn(config["freeze_bn"]["mortal"])
 
         self.optimizer = make_optimizer(mortal, dqn, aux_net, config["optim"])
@@ -215,7 +276,7 @@ class _Trainer:
         self.state_file, self.best_state_file = control["state_file"], control["best_state_file"]
         if path.exists(self.state_file):
             state = torch.load(self.state_file, weights_only=True, map_location=device)
-            logging.info(f"loaded: {datetime.fromtimestamp(state['timestamp']).strftime('%Y-%m-%d %H:%M:%S')}")
+            self.info(f"loaded: {datetime.fromtimestamp(state['timestamp']).strftime('%Y-%m-%d %H:%M:%S')}")
             load_mortal_state(mortal, state["mortal"])
             dqn.load_state_dict(state["current_dqn"])
             aux_net.load_state_dict(state["aux_net"])
@@ -225,8 +286,15 @@ class _Trainer:
             self.scaler.load_state_dict(state["scaler"])
             self.best_perf = state["best_perf"]
             self.total = state["steps"]
+        if self.world > 1:  # every rank starts from rank 0's weights and BatchNorm statistics (the rest is the same file)
+            import torch.distributed as dist
+
+            for m in (mortal, dqn, aux_net):
+                for t in m.state_dict().values():
+                    dist.broadcast(t, 0, group=self.group)
         self.optimizer.zero_grad(set_to_none=True)
-        logging.info(f"device: {device} ({torch.cuda.get_device_name(device)})")
+        self.info(f"device: {device} ({torch.cuda.get_device_name(device)})"
+                  + (f", rank {self.rank} of {self.world}" if self.world > 1 else ""))
 
         zero = lambda: torch.zeros((), dtype=torch.float64, device=device)
         self._zero = zero
@@ -236,9 +304,50 @@ class _Trainer:
         self.bad_steps = torch.zeros(self.save_every, dtype=torch.int32, device=device)
         self.idx = 0
 
+    def all_ranks(self, flag: bool) -> bool:
+        """True when `flag` holds on every rank (a host-side collective: no device synchronisation)"""
+        if self.world == 1:
+            return flag
+        import torch.distributed as dist
+
+        t = torch.tensor([int(flag)], dtype=torch.int32)
+        dist.all_reduce(t, op=dist.ReduceOp.MIN, group=self.flag_group)
+        return bool(t.item())
+
+    def _mean_over_ranks(self, *scalars):
+        """each device scalar averaged over the ranks (as they are with one rank)"""
+        if self.world == 1:
+            return scalars
+        import torch.distributed as dist
+
+        t = torch.stack([s.double() for s in scalars])
+        dist.all_reduce(t, group=self.group)
+        return (t / self.world).unbind()
+
+    def _all_reduce_grads(self):
+        """sum the gradients over the ranks (one flat all-reduce) and divide by the rank count: the gradient of the global
+        batch's mean loss, bit-identical on every rank"""
+        import torch.distributed as dist
+
+        grads = [p.grad for g in self.optimizer.param_groups for p in g["params"] if p.grad is not None]
+        flat = torch.cat([g.reshape(-1) for g in grads])
+        dist.all_reduce(flat, group=self.group)
+        flat /= self.world
+        o = 0
+        for g in grads:
+            g.copy_(flat[o:o + g.numel()].view_as(g))
+            o += g.numel()
+
     def check_actions(self):
-        """ValueError naming the first step since the last check whose batch had an action outside its mask"""
-        hit = torch.nonzero(self.bad_steps[:self.idx]).flatten().tolist()
+        """ValueError naming the first step since the last check whose batch had an action outside its mask (on any rank: every
+        rank raises the same error)"""
+        bad = self.bad_steps[:self.idx]
+        if self.world > 1:
+            import torch.distributed as dist
+
+            bad = bad.clone()
+            dist.all_reduce(bad, group=self.group)
+        hit = torch.nonzero(bad).flatten().tolist()
         if hit:
             raise ValueError(f"step {self.total - self.idx + hit[0] + 1}: an action of the batch is not legal in its mask")
 
@@ -246,7 +355,7 @@ class _Trainer:
         """one training step on a full batch, then the save and the test play when they are due"""
         mortal, dqn, aux_net = self.mortal, self.dqn, self.aux_net
         with torch.autocast(self.device.type, enabled=self.enable_amp):
-            phi = mortal.forward_train(obs)
+            phi = mortal.forward_train(obs, group=self.group)
             v, a = dqn.heads(phi)
             next_rank_logits, = aux_net(phi)
             dqn_loss, cql_loss, next_rank_loss, q, q_target, bad = train_ops.dqn_losses(
@@ -269,6 +378,8 @@ class _Trainer:
         self.total += 1
         self.idx += 1
         if self.idx % self.opt_step_every == 0:
+            if self.world > 1:
+                self._all_reduce_grads()
             if self.max_grad_norm > 0:
                 self.scaler.unscale_(self.optimizer)
                 clip_grad_norm_(chain.from_iterable(g["params"] for g in self.optimizer.param_groups), self.max_grad_norm)
@@ -285,15 +396,17 @@ class _Trainer:
         total, test_every, stats = self.total, self.test_every, self.stats
         self.check_actions()
         n = self.save_every
-        cql = "" if self.online else f" cql_loss {(stats['cql_loss'] / n).item():.6f}"
-        logging.info(f"steps {total:,}: dqn_loss {(stats['dqn_loss'] / n).item():.6f}{cql} "
-                     f"next_rank_loss {(stats['next_rank_loss'] / n).item():.6f} lr {self.scheduler.get_last_lr()[0]:.4e} "
-                     f"q {self.all_q.mean().item():.6f} q_target {self.all_q_target.mean().item():.6f}")
+        dqn_loss, cql_loss, next_rank_loss, q, q_target = self._mean_over_ranks(
+            stats["dqn_loss"], stats["cql_loss"], stats["next_rank_loss"], self.all_q.mean(), self.all_q_target.mean())
+        cql = "" if self.online else f" cql_loss {(cql_loss / n).item():.6f}"
+        self.info(f"steps {total:,}: dqn_loss {(dqn_loss / n).item():.6f}{cql} "
+                  f"next_rank_loss {(next_rank_loss / n).item():.6f} lr {self.scheduler.get_last_lr()[0]:.4e} "
+                  f"q {q.item():.6f} q_target {q_target.item():.6f}")
         for k in stats:
             stats[k] = self._zero()
         self.idx = 0
-        logging.info(f"total steps: {total:,} (~{(test_every - total % test_every) % test_every:,})")
-        state = {
+        self.info(f"total steps: {total:,} (~{(test_every - total % test_every) % test_every:,})")
+        state = None if self.rank else {
             "mortal": mortal_state_dict(self.mortal),
             "current_dqn": self.dqn.state_dict(),
             "aux_net": self.aux_net.state_dict(),
@@ -305,13 +418,14 @@ class _Trainer:
             "best_perf": self.best_perf,
             "config": self.config,
         }
-        torch.save(state, self.state_file)
+        if state is not None:
+            torch.save(state, self.state_file)
         if self.publish is not None and total % self.submit_every != 0:  # mortal/train.py:312-314
             self.publish(False)
 
         if total % test_every == 0:
             best_perf = self.best_perf
-            stat = self.test_player.test_play(self.test_games // 4, self.mortal, self.dqn, self.device)
+            stat = self.test_player.test_play(self.test_games // 4, self.mortal, self.dqn, self.device, group=self.group)
             self.mortal.train()
             self.dqn.train()
             avg_pt = stat.avg_pt([90, 45, 0, -135])  # for display only, never used in training
@@ -320,9 +434,9 @@ class _Trainer:
                 past_best = best_perf.copy()
                 best_perf["avg_pt"] = avg_pt
                 best_perf["avg_rank"] = stat.avg_rank
-            logging.info(f"avg rank: {stat.avg_rank:.6}")
-            logging.info(f"avg pt: {avg_pt:.6}")
-            logging.info("test play: rank 1/2/3/4 {:.4f} {:.4f} {:.4f} {:.4f}; agari {:.4f} houjuu {:.4f} fuuro {:.4f} "
+            self.info(f"avg rank: {stat.avg_rank:.6}")
+            self.info(f"avg pt: {avg_pt:.6}")
+            self.info("test play: rank 1/2/3/4 {:.4f} {:.4f} {:.4f} {:.4f}; agari {:.4f} houjuu {:.4f} fuuro {:.4f} "
                          "riichi {:.4f}; point per agari {:.1f} (riichi {:.1f}, fuuro {:.1f}, dama {:.1f}), per houjuu {:.1f}, "
                          "per round {:.1f}; jun agari {:.2f} houjuu {:.2f} riichi {:.2f}; after riichi agari {:.4f} houjuu "
                          "{:.4f}, chasing {:.4f}, chased {:.4f}, riichi point {:.1f}; after fuuro agari {:.4f} houjuu {:.4f}, "
@@ -334,7 +448,7 @@ class _Trainer:
                              stat.avg_riichi_jun, stat.agari_rate_after_riichi, stat.houjuu_rate_after_riichi,
                              stat.chasing_riichi_rate, stat.riichi_chased_rate, stat.avg_riichi_point,
                              stat.agari_rate_after_fuuro, stat.houjuu_rate_after_fuuro, stat.avg_fuuro_num, stat.avg_fuuro_point))
-            if better:
+            if better and state is not None:
                 torch.save(state, self.state_file)
                 logging.info(f"a new record has been made, pt: {past_best['avg_pt']:.4} -> {best_perf['avg_pt']:.4}, "
                              f"rank: {past_best['avg_rank']:.4} -> {best_perf['avg_rank']:.4}, saving to {self.best_state_file}")
@@ -351,29 +465,57 @@ def train(config, steps=None):
     """mortal/train.py train() over the whole config (dict), offline: one pass over the file list, as the reference runs. `steps`
     bounds this call to that many training steps (None: until the data ends). Returns (brain, dqn, aux_net, optimizer, total
     steps)."""
-    check_config(config)
+    world = world_info()[2]
+    check_config(config, world)
     T = _Trainer(config, online=False)
     ds = config["dataset"]
     grp = _load_grp(config)
     player_names_set = _player_names(ds)
-    logging.info(f"loaded {len(player_names_set):,} players")
-    file_list = _file_list(ds, player_names_set)
-    logging.info(f"file list size: {len(file_list):,}")
-    logging.info(f"total steps: {T.total:,} (~{(T.test_every - T.total % T.test_every) % T.test_every:,})")
+    T.info(f"loaded {len(player_names_set):,} players")
+    file_list = shard_file_list(ds, player_names_set, T) if world > 1 else _file_list(ds, player_names_set)
+    T.info(f"file list size: {len(file_list):,}")
+    T.info(f"total steps: {T.total:,} (~{(T.test_every - T.total % T.test_every) % T.test_every:,})")
     file_data = FileDatasetsIter(T.version, file_list, config["env"]["pts"], file_batch_size=ds["file_batch_size"],
                                  reserve_ratio=ds["reserve_ratio"], player_names=list(player_names_set), num_epochs=ds["num_epochs"],
                                  enable_augmentation=ds["enable_augmentation"], augmented_first=ds["augmented_first"], grp=grp,
                                  batch_size=T.batch_size, device=T.device.index)
     done = 0
-    for batch in file_data:
-        if steps is not None and done >= steps:
-            break
-        if batch[0].shape[0] != T.batch_size:
-            continue  # a final short batch is not trained on (mortal/train.py:389-422)
-        T.step(*batch)
-        done += 1
+    if world == 1:
+        for batch in file_data:
+            if steps is not None and done >= steps:
+                break
+            if batch[0].shape[0] != T.batch_size:
+                continue  # a final short batch is not trained on (mortal/train.py:389-422)
+            T.step(*batch)
+            done += 1
+    else:
+        batches = iter(file_data)
+        while steps is None or done < steps:
+            batch = next(batches, None)
+            # every rank steps or none does: training ends for all when one rank's shard runs out (its final short batch
+            # included, which is not trained on, as above)
+            if not T.all_ranks(batch is not None and batch[0].shape[0] == T.batch_size):
+                break
+            T.step(*batch)
+            done += 1
     T.check_actions()
     return T.mortal, T.dqn, T.aux_net, T.optimizer, T.total
+
+
+def shard_file_list(ds, player_names_set, T):
+    """this rank's shard of the file list: rank 0 builds or loads the index while the others wait, every rank loads it, rank 0
+    shuffles it and broadcasts the permutation, and each rank takes its contiguous block (ValueError on every rank when a block
+    would be empty)"""
+    import torch.distributed as dist
+
+    if T.rank == 0:
+        _file_list(ds, player_names_set)
+    dist.barrier(group=T.flag_group)
+    file_list = _file_list(ds, player_names_set)
+    check_shards(len(file_list), T.world)
+    perm = torch.randperm(len(file_list)) if T.rank == 0 else torch.empty(len(file_list), dtype=torch.int64)
+    dist.broadcast(perm, 0, group=T.flag_group)
+    return shard([file_list[i] for i in perm.tolist()], T.rank, T.world)
 
 
 def _train_pass(T, config, grp, games, steps, done):
@@ -405,7 +547,7 @@ def train_online(config, rounds=None, steps=None, monitor=None):
     from .player import TrainPlayer
     from .selfplay import SelfPlayGames
 
-    check_online_config(config)
+    check_online_config(config, world_info()[2])
     if config["online"].get("actor_devices"):
         from .online import train_concurrent
 
@@ -447,13 +589,28 @@ def train_online(config, rounds=None, steps=None, monitor=None):
 
 
 def main(argv=None):
+    """`python -m mortal_b200.train [CONFIG]`; under torchrun (WORLD_SIZE > 1) one data-parallel rank on cuda:LOCAL_RANK over NCCL"""
     argv = sys.argv[1:] if argv is None else argv
     logging.basicConfig(level=logging.INFO, format="%(asctime)s %(levelname)s %(message)s")
+    distributed = int(os.environ.get("WORLD_SIZE", "1")) > 1
     try:
         config = load_config(argv[0] if argv else None)
+        if distributed:
+            import torch.distributed as dist
+
+            device = torch.device("cuda", int(os.environ["LOCAL_RANK"]))
+            torch.cuda.set_device(device)
+            dist.init_process_group("nccl", device_id=device)
+            config["control"]["device"] = config["baseline"]["test"]["device"] = str(device)
         (train_online if config["control"].get("online", False) else train)(config)
     except KeyboardInterrupt:
         pass
+    finally:
+        if distributed:
+            import torch.distributed as dist
+
+            if dist.is_initialized():
+                dist.destroy_process_group()
 
 
 if __name__ == "__main__":

@@ -4,19 +4,34 @@ Activations are CUDA tensors logically [B, C, 1, L] in channels_last memory form
 AMP) or float16 (under `torch.autocast('cuda')`, whose default dtype is float16), with 1 <= C <= 256 and C % 8 == 0. The kernels
 compute in float32 and reduce in an order fixed by the shape, so two calls on the same inputs give bit-identical results.
 
-- `bn_mish(x, bn, frozen)`: BatchNorm1d + Mish of a pre-activation, train mode (batch statistics, running statistics updated as
-  nn.BatchNorm1d updates them) or frozen (running statistics, untouched).
+- `bn_mish(x, bn, frozen, group)`: BatchNorm1d + Mish of a pre-activation, train mode (batch statistics, running statistics updated
+  as nn.BatchNorm1d updates them) or frozen (running statistics, untouched). With a torch.distributed `group` of more than one
+  rank, train mode uses the statistics of the batch all the group's ranks hold together (synchronised BatchNorm).
 - `gate_residual(y, x, gate)`: ChannelGate(y) + x, the gate's shared MLP in torch (float32) on the pooled [B, C] vectors.
 - `dqn_losses(...)`: mortal/train.py:228-247 over the dueling head's v / a and the aux logits, in one launch.
 """
 from __future__ import annotations
 
 import ctypes as C
+import os
 
 import torch
 import torch.nn.functional as F
 
-from . import _lib
+from . import _cdecl, _lib
+
+HEADER = os.path.join(os.path.dirname(_cdecl.HEADER), "mjx_train_ranks.h")
+with open(HEADER) as _f:
+    SYMBOLS = _cdecl.functions(_f.read(), "mjx_")  # the entries of include/mjx_train_ranks.h, exported by libmjx.so
+_RANKS = None
+
+
+def ranks_lib():
+    """libmjx.so with the data-parallel BatchNorm entries of include/mjx_train_ranks.h bound"""
+    global _RANKS
+    if _RANKS is None:
+        _RANKS = _cdecl.bind(_lib.load(), SYMBOLS)
+    return _RANKS
 
 _DTYPES = {torch.float32: 0, torch.float16: 1}
 
@@ -64,18 +79,33 @@ def _scratch_floats(rows: int, c: int) -> int:
 
 class _BatchNormMish(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, weight, bias, running_mean, running_var, eps, momentum, training):
+    def forward(ctx, x, weight, bias, running_mean, running_var, eps, momentum, training, group):
         x, b, c, l = _nhwc(x)
         out = torch.empty_like(x)
         stats = torch.empty(3 * c, dtype=torch.float32, device=x.device)
         mean, invstd = stats[: 2 * c], stats[2 * c:]  # the batch mean as a float pair (hi, lo), and 1 / sqrt(var + eps)
         L = _lib.load()
         scratch = torch.empty(_scratch_floats(b * l, c), dtype=torch.float32, device=x.device)
-        _lib.check(L.mjx_train_bn_mish_fwd(_dtype_code(x), _p(x), _p(weight), _p(bias), _p(running_mean), _p(running_var), _p(mean),
-                                           _p(invstd), _p(out), b * l, c, float(eps), float(momentum), int(training), _p(scratch),
-                                           _stream(x)), "mjx_train_bn_mish_fwd")
+        if group is None:
+            _lib.check(L.mjx_train_bn_mish_fwd(_dtype_code(x), _p(x), _p(weight), _p(bias), _p(running_mean), _p(running_var),
+                                               _p(mean), _p(invstd), _p(out), b * l, c, float(eps), float(momentum), int(training),
+                                               _p(scratch), _stream(x)), "mjx_train_bn_mish_fwd")
+        else:
+            import torch.distributed as dist
+
+            L = ranks_lib()
+            rank, world = dist.get_rank(group), dist.get_world_size(group)
+            rows = torch.zeros((world, 3, c), dtype=torch.float64, device=x.device)  # (count, mean, M2) per rank
+            _lib.check(L.mjx_train_bn_local_stats(_dtype_code(x), _p(x), b * l, c, rank, world, _p(rows), _p(scratch), _stream(x)),
+                       "mjx_train_bn_local_stats")
+            # each rank wrote its own row into zeros: the SUM adds exact zeros, so this is a bit-exact all-gather (one that gloo
+            # also runs on CUDA tensors) and every rank merges the same rows
+            dist.all_reduce(rows, group=group)
+            _lib.check(L.mjx_train_bn_mish_fwd_ranks(_dtype_code(x), _p(x), _p(weight), _p(bias), _p(running_mean), _p(running_var),
+                                                     _p(mean), _p(invstd), _p(out), b * l, c, float(eps), float(momentum), _p(rows),
+                                                     world, _stream(x)), "mjx_train_bn_mish_fwd_ranks")
         ctx.save_for_backward(x, weight, bias, mean, invstd)
-        ctx.training = bool(training)
+        ctx.training, ctx.group = bool(training), group
         return out
 
     @staticmethod
@@ -88,24 +118,52 @@ class _BatchNormMish(torch.autograd.Function):
         dbeta = torch.empty_like(dgamma)
         L = _lib.load()
         scratch = torch.empty(_scratch_floats(b * l, c), dtype=torch.float32, device=x.device)
-        _lib.check(L.mjx_train_bn_mish_bwd(_dtype_code(x), _p(x), _p(dout), _p(weight), _p(bias), _p(mean), _p(invstd), _p(dx),
-                                           _p(dgamma), _p(dbeta), b * l, c, int(ctx.training), _p(scratch), _stream(x)),
-                   "mjx_train_bn_mish_bwd")
-        return dx, dgamma.to(weight.dtype), dbeta.to(bias.dtype), None, None, None, None, None
+        code, group = _dtype_code(x), ctx.group
+        if group is None:
+            _lib.check(L.mjx_train_bn_mish_bwd(code, _p(x), _p(dout), _p(weight), _p(bias), _p(mean), _p(invstd), _p(dx), _p(dgamma),
+                                               _p(dbeta), b * l, c, int(ctx.training), _p(scratch), _stream(x)), "mjx_train_bn_mish_bwd")
+        else:
+            import torch.distributed as dist
+
+            L = ranks_lib()
+            rank, world = dist.get_rank(group), dist.get_world_size(group)
+            sums = torch.zeros((world, 2, c), dtype=torch.float64, device=x.device)  # (sum dz, sum dz xhat) per rank
+            _lib.check(L.mjx_train_bn_bwd_local_sums(code, _p(x), _p(dout), _p(weight), _p(bias), _p(mean), _p(invstd), b * l, c, rank,
+                                                     world, _p(sums), _p(scratch), _stream(x)), "mjx_train_bn_bwd_local_sums")
+            dist.all_reduce(sums, group=group)  # the bit-exact all-gather of the forward's rows
+            # every rank holds b * l rows (bn_mish's condition); dgamma / dbeta are this rank's share
+            _lib.check(L.mjx_train_bn_mish_bwd_ranks(code, _p(x), _p(dout), _p(weight), _p(bias), _p(mean), _p(invstd), _p(dx),
+                                                     _p(dgamma), _p(dbeta), b * l, c, _p(sums), rank, world, world * b * l, _p(scratch),
+                                                     _stream(x)), "mjx_train_bn_mish_bwd_ranks")
+        return dx, dgamma.to(weight.dtype), dbeta.to(bias.dtype), None, None, None, None, None, None
 
 
-def bn_mish(x: torch.Tensor, bn: torch.nn.BatchNorm1d, frozen: bool = False) -> torch.Tensor:
+def bn_mish(x: torch.Tensor, bn: torch.nn.BatchNorm1d, frozen: bool = False, group=None) -> torch.Tensor:
     """mish(bn(x)) for x [B, C, 1, L] channels_last. Unless `frozen` or `bn` is in eval mode, the batch statistics are used and
-    bn's running_mean / running_var / num_batches_tracked are updated as nn.BatchNorm1d.forward in train mode updates them."""
+    bn's running_mean / running_var / num_batches_tracked are updated as nn.BatchNorm1d.forward in train mode updates them.
+
+    `group`: a torch.distributed process group whose every rank calls this with an x of the same shape, as data-parallel ranks
+    do. With more than one rank, training mode normalises with the statistics of all the ranks' rows together (exchanged twice
+    per forward and backward, in double), which every rank computes bit for bit alike, so the running statistics stay equal;
+    the parameter gradients are this rank's share, for the caller's gradient all-reduce to sum or average. None (or one rank):
+    this process's rows alone."""
     training = bn.training and not frozen
+    if group is not None:
+        import torch.distributed as dist
+
+        world = dist.get_world_size(group)
+        if world == 1 or not training:  # one rank, or the running statistics: nothing to exchange
+            group = None
+    else:
+        world = 1
     if training and bn.momentum is None:
         raise ValueError("bn_mish: a cumulative moving average (momentum=None) is not supported")
-    if training and x.shape[0] * x.shape[3] < 2:
+    if training and world * x.shape[0] * x.shape[3] < 2:
         raise ValueError("bn_mish: training-mode BatchNorm needs more than one value per channel")
     for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var):
         if t.dtype != torch.float32 or not t.is_contiguous():
             raise ValueError("bn_mish: the BatchNorm's parameters and statistics must be contiguous float32")
-    out = _BatchNormMish.apply(x, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps, bn.momentum or 0.0, training)
+    out = _BatchNormMish.apply(x, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps, bn.momentum or 0.0, training, group)
     if training:
         bn.num_batches_tracked.add_(1)
     return out
